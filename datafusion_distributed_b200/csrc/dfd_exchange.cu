@@ -8,13 +8,19 @@
 //           (src/worker/worker_connection_pool.rs:143-390)
 //   NetworkShuffleExec::execute: off = P*task_index, partition off+p from every
 //           producer (src/execution_plans/network_shuffle.rs:213-238)
-// with one worker per GPU and two transports:
+// with one worker per GPU and four transports:
 //   DFD_EXCHANGE_NCCL   partition locally, all-gather the T x N count matrix,
 //                       grouped ncclSend/ncclRecv per (column, destination).
 //   DFD_EXCHANGE_FUSED  the K2 scatter kernel stores every run straight into
 //                       the owner rank's receive window (CUDA-IPC mapped peer
 //                       memory over NVLink/NVSwitch): no staging buffer, no
 //                       separate send — compute and transfer are one kernel.
+//   single pass         (dfd_shuffle_device_onepass, fixed-width non-null) one
+//                       scatter kernel stores into fixed (partition, producer)
+//                       sub-windows; counts and completion are peer-memory flags.
+//   push                (dfd_shuffle_device_onepass for every other schema, and
+//                       dfd_exchange_gather) partition locally, then store each
+//                       destination's contiguous runs into the owner's window.
 // NCCL is resolved at run time (dlopen libnccl.so.2) so the single-GPU library
 // has no link-time dependency on it.
 #include <cuda_runtime.h>
@@ -336,9 +342,6 @@ struct dfd_exchange {
     int32_t* d_flags = nullptr;             // [0] my scatter overflowed a sub-window, [1] a peer never arrived
     int64_t* h_seg_counts = nullptr;        // pinned [T][P] rows producer r sent to my partition q
     int32_t* h_seg_flags = nullptr;         // pinned [T] overflow flags of the producers + [T] timed-out flag
-    bool pending_onepass = false;
-    bool pending_push = false;              // the last shuffle went through the push transport (already complete)
-    std::vector<int64_t> push_seg_starts, push_seg_counts;  // [P][T] result of the last push shuffle
     int64_t* d_meta = nullptr;              // device [XCHG_META_MAX] my metadata for the flag all-gather
     int64_t* h_meta = nullptr;              // pinned [MAX_RANKS][XCHG_META_MAX] gathered metadata
     void* d_runs = nullptr;                 // device PushRun array
@@ -350,15 +353,24 @@ struct dfd_exchange {
     size_t pev_pending = 0;
     double phase_ms[3] = {0, 0, 0};
     uint64_t phase_shuffles = 0;
-    int64_t pending_sub_cap = 0;
-    std::vector<dfd_column> last_in;        // retained for the exact (two-pass) re-run after an overflow
-    std::vector<dfd_column> last_out;
-    dfd_partitioner* last_part = nullptr;
-    int64_t last_rows = 0;
     uint64_t onepass_fallbacks = 0;
-    bool pending_async = false;       // a fused shuffle has been enqueued but not waited for
-    size_t pending_row_bytes = 0;
-    uint32_t pending_P = 0;
+    // What dfd_exchange_collect / _wait / _pending_segments report on: the last shuffle, if it left a result to pick up.
+    // Every shuffle entry point resets it to NONE first and sets its own kind only on success.
+    struct Pending {
+        enum Kind {
+            NONE,
+            DENSE,     // two-pass fused shuffle enqueued, not yet waited for
+            REGIONS,   // single-pass shuffle enqueued: (partition, producer) sub-windows
+            SEGMENTS,  // push transport: already complete, collectable until the next shuffle starts
+        } kind = NONE;
+        uint32_t P = 0;
+        size_t row_bytes = 0;
+        int64_t sub_cap = 0;                  // REGIONS: rows per sub-window
+        std::vector<dfd_column> in;           // REGIONS: the input, kept for the exact two-pass re-run after an overflow
+        dfd_partitioner* part = nullptr;
+        int64_t rows = 0;
+        std::vector<int64_t> seg_starts, seg_counts;  // SEGMENTS
+    } pending;
     // host pipeline (dfd_shuffle_host): H2D | shuffle | D2H of consecutive chunks overlap
     cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
     cudaEvent_t e_h2d[2] = {}, e_k[2] = {}, e_d2h[2] = {};
@@ -517,6 +529,24 @@ static int ensure_count_buffers(dfd_exchange* x, uint32_t N) {
     return DFD_OK;
 }
 
+// Checks and set-up shared by the shuffle entry points.  On success `lk` holds the context's lock, the device is set, the
+// count buffers fit, the shuffle is counted and nothing is pending any more.
+static int begin_shuffle(dfd_exchange* x, dfd_partitioner* part, const dfd_column* in_cols, const dfd_column* out_cols, uint32_t P,
+                         const char* fn, std::unique_lock<std::mutex>& lk) {
+    if (!x || !part || !in_cols || !out_cols) return set_error(DFD_ERR_INVALID_ARGUMENT, "%s: NULL argument", fn);
+    dfd_ctx* c = x->ctx;
+    if (part->ctx != c) return set_error(DFD_ERR_INVALID_ARGUMENT, "partitioner and exchange belong to different contexts");
+    if (P < 1 || (uint64_t)P * x->world != part->N)
+        return set_error(DFD_ERR_INVALID_ARGUMENT, "num_partitions %u != partitions_per_task %u x %d workers", part->N, P, x->world);
+    lk = std::unique_lock<std::mutex>(c->mu);
+    x->pending.kind = dfd_exchange::Pending::NONE;
+    CUDA_TRY(cudaSetDevice(c->device), "cudaSetDevice");
+    int rc = ensure_count_buffers(x, part->N);
+    if (rc) return rc;
+    x->shuffles++;
+    return DFD_OK;
+}
+
 /* Allocate this rank's receive window and map every peer's (collective call). */
 int dfd_exchange_setup_window(dfd_exchange* x, size_t window_bytes) {
     if (!x) return set_error(DFD_ERR_INVALID_ARGUMENT, "NULL exchange");
@@ -589,20 +619,41 @@ static size_t row_bytes_of(const dfd_column* cols, int n_cols) {
     return rb;
 }
 
-// Fused shuffle of device columns into window slot `slot` of `n_slots` (the window is split so
-// that a chunked host pipeline can drain one slot while the next chunk lands in the other).
-// Ends with a stream synchronize: x->h_my_starts holds this worker's part_starts[P+1].
-// `e_k`, if given, is recorded right after the last kernel / barrier of this shuffle.
-static int fused_shuffle_finish(dfd_exchange* x, uint32_t P) {
-    dfd_ctx* c = x->ctx;
-    CUDA_TRY(cudaStreamSynchronize(c->stream), "fused shuffle");
-    x->pending_async = false;
+// Window slot `slot` of `n_slots` of the fused transports (the window is split so that a chunked host pipeline can drain one
+// slot while the next chunk lands in the other).  Identical on every rank: capacity rounded down to `row_align` rows, column
+// i at byte offset capacity * sum(width[0..i)).  outs: the columns as the peer scatter sees them (values = byte offset into
+// every rank's slot, peer_base[r]); out_cols: this rank's own slot.  Returns the capacity in rows.
+static int64_t layout_window_slot(const dfd_exchange* x, const dfd_column* in_cols, int n_cols, size_t rb, int slot, int n_slots,
+                                  int64_t row_align, void** peer_base, std::vector<dfd_column>& outs, dfd_column* out_cols) {
+    const size_t slot_bytes = (x->window_bytes / (size_t)n_slots) & ~(size_t)255;
+    const int64_t capacity_rows = (int64_t)(slot_bytes / rb) / row_align * row_align;
+    for (int r = 0; r < x->world; ++r) peer_base[r] = (char*)x->peer_window[r] + XCHG_HEADER_BYTES + (size_t)slot * slot_bytes;
+    outs.resize(n_cols);
+    size_t off = 0;
+    for (int i = 0; i < n_cols; ++i) {
+        outs[i] = in_cols[i];
+        outs[i].validity = nullptr;
+        outs[i].offset = 0;
+        out_cols[i] = outs[i];
+        outs[i].values = (void*)off;
+        out_cols[i].values = (char*)peer_base[x->rank] + off;
+        off += (size_t)capacity_rows * (size_t)in_cols[i].width;
+    }
+    return capacity_rows;
+}
+
+// Completes a two-pass fused shuffle with a stream synchronize: x->h_my_starts then holds this worker's part_starts[P+1].
+static int fused_shuffle_finish(dfd_exchange* x, uint32_t P, size_t rb) {
+    CUDA_TRY(cudaStreamSynchronize(x->ctx->stream), "fused shuffle");
     if (*x->h_abort)
         return set_error(DFD_ERR_CAPACITY, "a receive window slot is too small for this shuffle (window %zu B)", x->window_bytes);
-    x->bytes_received += (uint64_t)x->h_my_starts[P] * x->pending_row_bytes;
+    x->bytes_received += (uint64_t)x->h_my_starts[P] * rb;
     return DFD_OK;
 }
 
+// Two-pass fused shuffle of device columns into window slot `slot` of `n_slots`.  With `sync` it completes inside the call;
+// without, it stays pending (DENSE) for dfd_exchange_wait / _collect.  `e_k`, if given, is recorded right after the last
+// kernel / barrier of this shuffle.
 static int fused_shuffle_locked(dfd_exchange* x, dfd_partitioner* part, const dfd_column* in_cols, int n_cols, int64_t n_rows,
                                 uint32_t P, int slot, int n_slots, dfd_column* out_cols, cudaEvent_t e_k, bool sync = true) {
     dfd_ctx* c = x->ctx;
@@ -613,24 +664,9 @@ static int fused_shuffle_locked(dfd_exchange* x, dfd_partitioner* part, const df
     if (!x->window_ready) return set_error(DFD_ERR_INVALID_ARGUMENT, "fused exchange needs dfd_exchange_setup_window first");
     const size_t rb = row_bytes_of(in_cols, n_cols);
     if (rb == 0) return set_error(DFD_ERR_INVALID_ARGUMENT, "no fixed-width columns");
-    const size_t slot_bytes = (x->window_bytes / (size_t)n_slots) & ~(size_t)255;
-    const int64_t capacity_rows = (int64_t)(slot_bytes / rb) / 16 * 16;
     void* peer_base[MAX_RANKS];
-    for (int r = 0; r < T; ++r) peer_base[r] = (char*)x->peer_window[r] + XCHG_HEADER_BYTES + (size_t)slot * slot_bytes;
-    // slot layout (identical on every rank): column c at byte offset capacity_rows * sum(width[0..c))
-    std::vector<dfd_column> outs(n_cols);
-    size_t off = 0;
-    for (int i = 0; i < n_cols; ++i) {
-        outs[i] = in_cols[i];
-        outs[i].values = (void*)off;  // peer mode: byte offset into every window slot
-        outs[i].validity = nullptr;
-        outs[i].offset = 0;
-        out_cols[i] = in_cols[i];
-        out_cols[i].values = (char*)peer_base[x->rank] + off;
-        out_cols[i].validity = nullptr;
-        out_cols[i].offset = 0;
-        off += (size_t)capacity_rows * (size_t)in_cols[i].width;
-    }
+    std::vector<dfd_column> outs;
+    const int64_t capacity_rows = layout_window_slot(x, in_cols, n_cols, rb, slot, n_slots, 16, peer_base, outs, out_cols);
     int rc;
     PartitionJob job;
     if ((rc = job.prepare(part, in_cols, n_cols, n_rows, outs.data(), true, s))) return rc;
@@ -650,11 +686,11 @@ static int fused_shuffle_locked(dfd_exchange* x, dfd_partitioner* part, const df
     CUDA_TRY(cudaMemcpyAsync(x->h_my_starts, x->d_my_starts, sizeof(int64_t) * (P + 1), cudaMemcpyDeviceToHost, s), "D2H starts");
     CUDA_TRY(cudaMemcpyAsync(x->h_abort, x->d_abort, sizeof(int32_t), cudaMemcpyDeviceToHost, s), "D2H flag");
     x->bytes_sent += (uint64_t)n_rows * rb;
-    x->pending_row_bytes = rb;
-    x->pending_async = true;
-    x->pending_P = P;
-    (void)capacity_rows;
-    return sync ? fused_shuffle_finish(x, P) : DFD_OK;
+    if (sync) return fused_shuffle_finish(x, P, rb);
+    x->pending.kind = dfd_exchange::Pending::DENSE;
+    x->pending.P = P;
+    x->pending.row_bytes = rb;
+    return DFD_OK;
 }
 
 // ---- single-pass fused shuffle ------------------------------------------------------------------
@@ -666,12 +702,10 @@ static int fused_shuffle_locked(dfd_exchange* x, dfd_partitioner* part, const df
 // particular inter-producer order (src/execution_plans/network_shuffle.rs:230-237 `select_all`).
 // (decided from the SCHEMA — column kinds and the nullable flags the caller passes in out_cols[].validity — so that every
 //  worker takes the same transport whether or not its own rows contain nulls)
-static bool onepass_supported(const dfd_exchange* x, const dfd_partitioner* part, const dfd_column* cols, const dfd_column* out_cols, int n_cols,
-                              uint32_t P) {
+static bool onepass_supported(const dfd_partitioner* part, const dfd_column* cols, const dfd_column* out_cols, int n_cols, uint32_t P) {
     if (part->N > ONEPASS_MAX_N || P > XCHG_MAX_P || n_cols < 1) return false;
     for (int i = 0; i < n_cols; ++i)
         if (cols[i].kind != DFD_COL_FIXED || cols[i].validity || out_cols[i].validity) return false;
-    (void)x;
     return true;
 }
 
@@ -682,25 +716,11 @@ static int onepass_shuffle_locked(dfd_exchange* x, dfd_partitioner* part, const 
     cudaStream_t s = c->stream;
     if (!x->window_ready) return set_error(DFD_ERR_INVALID_ARGUMENT, "fused exchange needs dfd_exchange_setup_window first");
     const size_t rb = row_bytes_of(in_cols, n_cols);
-    const size_t slot_bytes = (x->window_bytes / (size_t)n_slots) & ~(size_t)255;
-    const int64_t capacity_rows = (int64_t)(slot_bytes / rb) / 32 * 32;
+    void* peer_base[MAX_RANKS];
+    std::vector<dfd_column> outs;
+    const int64_t capacity_rows = layout_window_slot(x, in_cols, n_cols, rb, slot, n_slots, 32, peer_base, outs, out_cols);
     const int64_t sub_cap = capacity_rows / ((int64_t)P * T) / 32 * 32;  // rows per (partition, producer) sub-window
     if (sub_cap < 32) return set_error(DFD_ERR_CAPACITY, "receive window (%zu B) too small for %u x %d sub-windows", x->window_bytes, P, T);
-    void* peer_base[MAX_RANKS];
-    for (int r = 0; r < T; ++r) peer_base[r] = (char*)x->peer_window[r] + XCHG_HEADER_BYTES + (size_t)slot * slot_bytes;
-    std::vector<dfd_column> outs(n_cols);
-    size_t off = 0;
-    for (int i = 0; i < n_cols; ++i) {
-        outs[i] = in_cols[i];
-        outs[i].values = (void*)off;  // peer mode: byte offset into every window slot
-        outs[i].validity = nullptr;
-        outs[i].offset = 0;
-        out_cols[i] = in_cols[i];
-        out_cols[i].values = (char*)peer_base[x->rank] + off;
-        out_cols[i].validity = nullptr;
-        out_cols[i].offset = 0;
-        off += (size_t)capacity_rows * (size_t)in_cols[i].width;
-    }
     const unsigned long long epoch = ++x->epoch;
     ExchangeHeader* hdr = (ExchangeHeader*)x->window;
     cudaEvent_t* pe = nullptr;
@@ -755,10 +775,14 @@ static int onepass_shuffle_locked(dfd_exchange* x, dfd_partitioner* part, const 
     CUDA_TRY(cudaMemcpyAsync(x->h_seg_flags, hdr->overflow, sizeof(int32_t) * (size_t)T, cudaMemcpyDeviceToHost, s), "D2H overflow flags");
     CUDA_TRY(cudaMemcpyAsync(x->h_seg_flags + MAX_RANKS, x->d_flags + 1, sizeof(int32_t), cudaMemcpyDeviceToHost, s), "D2H timeout flag");
     x->bytes_sent += (uint64_t)n_rows * rb;
-    x->pending_row_bytes = rb;
-    x->pending_onepass = true;
-    x->pending_P = P;
-    x->pending_sub_cap = sub_cap;
+    dfd_exchange::Pending& pd = x->pending;
+    pd.kind = dfd_exchange::Pending::REGIONS;
+    pd.P = P;
+    pd.row_bytes = rb;
+    pd.sub_cap = sub_cap;
+    pd.in.assign(in_cols, in_cols + n_cols);
+    pd.part = part;
+    pd.rows = n_rows;
     return DFD_OK;
 }
 
@@ -824,6 +848,33 @@ struct PushCol {
     int64_t offset;  // Arrow logical offset of the source column
 };
 
+size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// How the push transport and NCCL mode move column i: kind, offset width, index among the string columns, and whether a
+// validity lane travels — the SCHEMA's flag (out_cols[i].validity != NULL on entry, the same on every worker) or a bitmap
+// in this worker's input.  values / offsets / validity / offset describe in_cols[i].
+int describe_columns(const dfd_column* in_cols, const dfd_column* out_cols, int n_cols, std::vector<PushCol>& pc) {
+    pc.assign(n_cols, PushCol{});
+    int V = 0;
+    for (int i = 0; i < n_cols; ++i) {
+        const dfd_column& ic = in_cols[i];
+        PushCol& q = pc[i];
+        q.kind = ic.kind; q.width = ic.width; q.ow = ic.kind == DFD_COL_LARGE_UTF8 ? 8 : 4; q.var_index = -1;
+        if (ic.kind == DFD_COL_UTF8 || ic.kind == DFD_COL_LARGE_UTF8 || ic.kind == DFD_COL_BINARY) q.var_index = V++;
+        else if (ic.kind != DFD_COL_FIXED && ic.kind != DFD_COL_BOOL) return set_error(DFD_ERR_UNSUPPORTED, "column %d: unknown column kind %d", i, ic.kind);
+        q.in_valid = ic.validity != nullptr;
+        q.nullable = out_cols[i].validity != nullptr || q.in_valid;
+        q.values = (const char*)ic.values; q.offsets = (const char*)ic.offsets; q.validity = (const char*)ic.validity; q.offset = ic.offset;
+    }
+    return DFD_OK;
+}
+
+int n_var_cols(const std::vector<PushCol>& pc) {
+    int V = 0;
+    for (const PushCol& q : pc) V += q.var_index >= 0;
+    return V;
+}
+
 __global__ void k_slice_rows(const int64_t* __restrict__ starts, uint32_t n, int64_t* __restrict__ rows) {
     for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < n; g += gridDim.x * blockDim.x) rows[g] = starts[g + 1] - starts[g];
 }
@@ -837,9 +888,7 @@ static int push_slices_locked(dfd_exchange* x, const std::vector<PushCol>& pc, c
     const int T = x->world;
     const int n_cols = (int)pc.size();
     cudaStream_t s = c->stream;
-    auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    int V = 0;
-    for (const PushCol& q : pc) V += q.var_index >= 0;
+    const int V = n_var_cols(pc);
     const uint32_t NS = R.n_slices();
     const uint32_t n_meta = (uint32_t)(1 + V) * NS;
     if (n_meta > XCHG_META_MAX)
@@ -1004,64 +1053,50 @@ static int push_slices_locked(dfd_exchange* x, const std::vector<PushCol>& pc, c
         out_cols[i].values_bytes = 0;
     }
     const uint32_t nseg = R.n_segments(x->rank);
-    x->push_seg_starts.assign(nseg, 0);
-    x->push_seg_counts.assign(nseg, 0);
+    dfd_exchange::Pending& pd = x->pending;
+    pd.seg_starts.assign(Me.seg_start.begin(), Me.seg_start.end());
+    pd.seg_counts.assign(nseg, 0);
     uint64_t rows = 0;
     for (uint32_t sg = 0; sg < nseg; ++sg) {
         int r;
         uint32_t g;
         R.source(x->rank, sg, &r, &g);
-        x->push_seg_starts[sg] = Me.seg_start[sg];
-        x->push_seg_counts[sg] = r >= 0 ? rows_of(r, g) : 0;
-        rows += (uint64_t)x->push_seg_counts[sg];
+        pd.seg_counts[sg] = r >= 0 ? rows_of(r, g) : 0;
+        rows += (uint64_t)pd.seg_counts[sg];
     }
     for (int i = 0; i < n_cols; ++i)
         if (pc[i].kind == DFD_COL_FIXED) x->bytes_received += rows * (uint64_t)pc[i].width;
     x->push_shuffles++;
-    x->pending_push = true;
-    x->pending_onepass = false;
-    x->pending_async = false;
+    pd.kind = dfd_exchange::Pending::SEGMENTS;
     return DFD_OK;
 }
 
-static int push_shuffle_locked(dfd_exchange* x, dfd_partitioner* part, const dfd_column* in_cols, int n_cols, int64_t n_rows, uint32_t P,
-                               dfd_column* out_cols) {
+// Local partition (K1/K1b/K2 + K4) of in_cols into a destination-sorted copy in x->send, for the push transport and NCCL
+// mode: destination g is rows [part->d_part_starts[g], part->d_part_starts[g + 1]) of every staged column, and pc (from
+// describe_columns) is pointed at the copies.  The `extra_bytes` behind them are the caller's (*extra).  *d_totals: rows per
+// destination.
+static int stage_locally(dfd_exchange* x, dfd_partitioner* part, const dfd_column* in_cols, int n_cols, int64_t n_rows, std::vector<PushCol>& pc,
+                         size_t extra_bytes, char** extra, const int64_t** d_totals) {
     dfd_ctx* c = x->ctx;
-    const uint32_t N = part->N;
-    cudaStream_t s = c->stream;
-    if (!x->window_ready) return set_error(DFD_ERR_INVALID_ARGUMENT, "fused exchange needs dfd_exchange_setup_window first");
-    auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    std::vector<PushCol> pc(n_cols);
     std::vector<size_t> st_values(n_cols), st_off(n_cols), st_valid(n_cols);
     std::vector<int64_t> cap_bytes(n_cols, 0);
-    int V = 0;
     size_t stage_bytes = 0;
     const size_t bm = al((size_t)((n_rows + 63) / 64 * 8 + 16));
     for (int i = 0; i < n_cols; ++i) {
-        const dfd_column& ic = in_cols[i];
-        PushCol& q = pc[i];
-        q = PushCol{};
-        q.kind = ic.kind; q.width = ic.width; q.ow = ic.kind == DFD_COL_LARGE_UTF8 ? 8 : 4; q.var_index = -1;
-        q.in_valid = ic.validity != nullptr;
-        q.nullable = out_cols[i].validity != nullptr || q.in_valid;  // (the schema's flag: every worker passes the same)
-        if (ic.kind == DFD_COL_FIXED) {
-            st_values[i] = stage_bytes; stage_bytes += al((size_t)n_rows * ic.width + 16);
-        } else if (ic.kind == DFD_COL_BOOL) {
+        const PushCol& q = pc[i];
+        if (q.kind == DFD_COL_FIXED) {
+            st_values[i] = stage_bytes; stage_bytes += al((size_t)n_rows * q.width + 16);
+        } else if (q.kind == DFD_COL_BOOL) {
             st_values[i] = stage_bytes; stage_bytes += bm;
-        } else if (ic.kind == DFD_COL_UTF8 || ic.kind == DFD_COL_LARGE_UTF8 || ic.kind == DFD_COL_BINARY) {
-            q.var_index = V++;
-            cap_bytes[i] = ic.values_bytes > 0 ? ic.values_bytes : 16;
+        } else {
+            cap_bytes[i] = in_cols[i].values_bytes > 0 ? in_cols[i].values_bytes : 16;
             st_off[i] = stage_bytes; stage_bytes += al((size_t)(n_rows + 1) * q.ow + 16);
             st_values[i] = stage_bytes; stage_bytes += al((size_t)cap_bytes[i] + 16);
-        } else {
-            return set_error(DFD_ERR_UNSUPPORTED, "column %d: unknown column kind %d", i, ic.kind);
         }
         if (q.in_valid) { st_valid[i] = stage_bytes; stage_bytes += bm; }
     }
-    const size_t scratch_off = stage_bytes;
-    stage_bytes += al((size_t)(V + 1) * N * 8 + 64);
     int rc;
-    if ((rc = x->send.ensure(stage_bytes + 256, c->device))) return rc;
+    if ((rc = x->send.ensure(stage_bytes + extra_bytes + 256, c->device))) return rc;
     char* sb = (char*)x->send.ptr;
     std::vector<dfd_column> staged(n_cols);
     for (int i = 0; i < n_cols; ++i) {
@@ -1072,18 +1107,30 @@ static int push_shuffle_locked(dfd_exchange* x, dfd_partitioner* part, const dfd
         staged[i].validity = q.in_valid ? (uint8_t*)(sb + st_valid[i]) : nullptr;
         staged[i].offset = 0;
         staged[i].values_bytes = cap_bytes[i];
-        q.values = sb + st_values[i];
-        q.offsets = q.var_index >= 0 ? sb + st_off[i] : nullptr;
-        q.validity = q.in_valid ? sb + st_valid[i] : nullptr;
+        q.values = (const char*)staged[i].values;
+        q.offsets = (const char*)staged[i].offsets;
+        q.validity = (const char*)staged[i].validity;
         q.offset = 0;
     }
     PartitionJob job;
-    if ((rc = job.prepare(part, in_cols, n_cols, n_rows, staged.data(), false, s))) return rc;
+    if ((rc = job.prepare(part, in_cols, n_cols, n_rows, staged.data(), false, c->stream))) return rc;
     if ((rc = job.run_hist_scan())) return rc;
     if ((rc = job.run_scatter(part->d_part_starts, nullptr, 1, 1, nullptr))) return rc;
-    Route R{DFD_ROUTE_SHUFFLE, P, x->world, x->world};
-    x->pending_P = P;
-    return push_slices_locked(x, pc, in_cols, R, part->d_part_starts, sb + scratch_off, out_cols);
+    *extra = sb + stage_bytes;
+    *d_totals = job.d_totals;
+    return DFD_OK;
+}
+
+static int push_shuffle_locked(dfd_exchange* x, dfd_partitioner* part, const dfd_column* in_cols, int n_cols, int64_t n_rows, uint32_t P,
+                               dfd_column* out_cols) {
+    if (!x->window_ready) return set_error(DFD_ERR_INVALID_ARGUMENT, "fused exchange needs dfd_exchange_setup_window first");
+    std::vector<PushCol> pc;
+    char* scratch;
+    const int64_t* d_totals;
+    int rc = describe_columns(in_cols, out_cols, n_cols, pc);
+    if (rc == DFD_OK) rc = stage_locally(x, part, in_cols, n_cols, n_rows, pc, al((size_t)(n_var_cols(pc) + 1) * part->N * 8 + 64), &scratch, &d_totals);
+    if (rc) return rc;
+    return push_slices_locked(x, pc, in_cols, Route{DFD_ROUTE_SHUFFLE, P, x->world, x->world}, part->d_part_starts, scratch, out_cols);
 }
 
 /* The shuffle: producer task `rank` holds n_rows local rows; afterwards this
@@ -1093,22 +1140,16 @@ static int push_shuffle_locked(dfd_exchange* x, dfd_partitioner* part, const dfd
 int dfd_shuffle_device(dfd_exchange* x, dfd_partitioner* part, int mode, const dfd_column* in_cols, int n_cols,
                        int64_t n_rows, uint32_t partitions_per_task, dfd_column* out_cols, int64_t out_capacity_rows,
                        int64_t* part_starts_host) {
-    if (!x || !part || !in_cols || !out_cols || !part_starts_host)
-        return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_shuffle_device: NULL argument");
-    dfd_ctx* c = x->ctx;
-    if (part->ctx != c) return set_error(DFD_ERR_INVALID_ARGUMENT, "partitioner and exchange belong to different contexts");
+    if (!part_starts_host) return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_shuffle_device: NULL argument");
     const uint32_t P = partitions_per_task;
+    std::unique_lock<std::mutex> lk;
+    int rc = begin_shuffle(x, part, in_cols, out_cols, P, "dfd_shuffle_device", lk);
+    if (rc) return rc;
+    dfd_ctx* c = x->ctx;
     const uint32_t N = part->N;
     const int T = x->world;
-    if (P < 1 || (uint64_t)P * T != N)
-        return set_error(DFD_ERR_INVALID_ARGUMENT, "num_partitions %u != partitions_per_task %u x %d workers", N, P, T);
     NcclApi* n = T > 1 ? nccl_api() : nullptr;
-    std::lock_guard<std::mutex> lk(c->mu);
-    CUDA_TRY(cudaSetDevice(c->device), "cudaSetDevice");
-    int rc = ensure_count_buffers(x, N);
-    if (rc) return rc;
     cudaStream_t s = c->stream;
-    x->shuffles++;
 
     if (mode == DFD_EXCHANGE_FUSED) {
         rc = fused_shuffle_locked(x, part, in_cols, n_cols, n_rows, P, 0, 1, out_cols, nullptr);
@@ -1122,100 +1163,65 @@ int dfd_shuffle_device(dfd_exchange* x, dfd_partitioner* part, int mode, const d
     // Every column kind the local partitioner supports travels: fixed-width values as they are,
     // bitmaps (validity, booleans) as one byte per row, strings as (lengths, bytes); the receiver
     // rebuilds bitmaps and offsets (k_bytes_to_bits, lengths -> offsets scan).
-    auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    struct XCol {
-        int kind, width, ow;
-        bool has_valid;   // the column travels with a validity lane (decided by the OUTPUT descriptor, i.e. the schema,
-                          // so that every worker agrees even if its own rows happen to contain no nulls)
-        bool in_valid;    // this worker's input actually carries a validity bitmap
-        size_t st_values, st_valid, st_off;        // staging offsets (destination-sorted local output)
-        size_t cv_valid, cv_values, cv_len;        // sender-side conversions (u8 per row / lengths)
-        size_t rv_valid, rv_values, rv_len;        // receiver-side temporaries
-        int64_t cap_bytes;                          // var-width: staging byte capacity
-    };
-    std::vector<XCol> xc(n_cols);
-    size_t stage_bytes = 0;
+    std::vector<PushCol> pc;
+    if ((rc = describe_columns(in_cols, out_cols, n_cols, pc))) return rc;
     for (int i = 0; i < n_cols; ++i) {
-        const dfd_column& ic = in_cols[i];
-        XCol& c0 = xc[i];
-        c0 = XCol{};
-        c0.kind = ic.kind; c0.width = ic.width; c0.ow = ic.kind == DFD_COL_LARGE_UTF8 ? 8 : 4;
-        c0.in_valid = ic.validity != nullptr;
-        c0.has_valid = out_cols[i].validity != nullptr;
-        if (out_cols[i].kind != ic.kind || out_cols[i].width != ic.width || !out_cols[i].values)
+        const dfd_column& oc = out_cols[i];
+        if (oc.kind != in_cols[i].kind || oc.width != in_cols[i].width || !oc.values)
             return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: out layout mismatch", i);
-        if (c0.in_valid && !c0.has_valid)
+        if (pc[i].in_valid && !oc.validity)
             return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: input has nulls but out validity is NULL (nullable columns need a validity "
                                                        "buffer on EVERY worker)", i);
-        const size_t bm = al((size_t)((n_rows + 63) / 64 * 8 + 8));
-        if (ic.kind == DFD_COL_FIXED) {
-            c0.st_values = stage_bytes; stage_bytes += al((size_t)n_rows * ic.width + 16);
-        } else if (ic.kind == DFD_COL_BOOL) {
-            c0.st_values = stage_bytes; stage_bytes += bm;
-            c0.cv_values = stage_bytes; stage_bytes += al((size_t)n_rows + 16);
-        } else if (ic.kind == DFD_COL_UTF8 || ic.kind == DFD_COL_LARGE_UTF8 || ic.kind == DFD_COL_BINARY) {
-            if (!out_cols[i].offsets) return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: out offsets is NULL", i);
-            c0.cap_bytes = ic.values_bytes > 0 ? ic.values_bytes : 16;
-            c0.st_off = stage_bytes; stage_bytes += al((size_t)(n_rows + 1) * c0.ow + 16);
-            c0.st_values = stage_bytes; stage_bytes += al((size_t)c0.cap_bytes + 16);
-            c0.cv_len = stage_bytes; stage_bytes += al((size_t)(n_rows + 1) * c0.ow + 16);
-        } else {
-            return set_error(DFD_ERR_UNSUPPORTED, "column %d: unknown column kind %d", i, ic.kind);
-        }
-        if (c0.in_valid) { c0.st_valid = stage_bytes; stage_bytes += bm; }
-        if (c0.has_valid) { c0.cv_valid = stage_bytes; stage_bytes += al((size_t)n_rows + 16); }
+        if (pc[i].var_index >= 0 && !oc.offsets) return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: out offsets is NULL", i);
     }
-    const size_t meta_off = stage_bytes;               // per var column: bytes[N] | first[N] (device)
-    stage_bytes += al((size_t)n_cols * 2 * N * 8 + 64);
-    if ((rc = x->send.ensure(stage_bytes + 256, c->device))) return rc;
-    char* sb = (char*)x->send.ptr;
-    std::vector<dfd_column> staged(n_cols);
+    // After these checks pc[i].nullable == (out_cols[i].validity != NULL), the schema's flag: every worker sends the same lanes.
+    // Conversion buffers, u8 per row: the "values lane" (a boolean column's values, a string column's lengths) and the
+    // validity lane, on the sender behind the staged columns and on the receiver in x->recv_tmp.
+    struct Conv { size_t send_values, send_valid, recv_values, recv_valid; };
+    std::vector<Conv> cv(n_cols);
+    auto lane_width = [](const PushCol& q) { return q.kind == DFD_COL_BOOL ? (size_t)1 : (size_t)q.ow; };
+    const size_t V = (size_t)n_var_cols(pc);
+    size_t conv_bytes = 0;
     for (int i = 0; i < n_cols; ++i) {
-        const XCol& c0 = xc[i];
-        staged[i] = in_cols[i];
-        staged[i].values = sb + c0.st_values;
-        staged[i].offsets = c0.kind >= DFD_COL_UTF8 ? (void*)(sb + c0.st_off) : nullptr;
-        staged[i].validity = c0.in_valid ? (uint8_t*)(sb + c0.st_valid) : nullptr;
-        staged[i].offset = 0;
-        staged[i].values_bytes = c0.cap_bytes;
-        const size_t bm = (size_t)((n_rows + 63) / 64 * 8 + 8);
-        if (c0.kind == DFD_COL_BOOL) CUDA_TRY(cudaMemsetAsync(sb + c0.st_values, 0, bm, s), "memset");
-        if (c0.in_valid) CUDA_TRY(cudaMemsetAsync(sb + c0.st_valid, 0, bm, s), "memset");
+        const PushCol& q = pc[i];
+        if (q.kind != DFD_COL_FIXED) { cv[i].send_values = conv_bytes; conv_bytes += al((size_t)(n_rows + 1) * lane_width(q) + 16); }
+        if (q.nullable) { cv[i].send_valid = conv_bytes; conv_bytes += al((size_t)n_rows + 16); }
     }
-    PartitionJob job;
-    if ((rc = job.prepare(part, in_cols, n_cols, n_rows, staged.data(), false, s))) return rc;
-    if ((rc = job.run_hist_scan())) return rc;
-    if ((rc = job.run_scatter(part->d_part_starts, nullptr, 1, 1, nullptr))) return rc;
+    const size_t meta_off = conv_bytes;  // per string column: bytes[N] | first[N] (device)
+    conv_bytes += al(V * 2 * N * 8 + 64);
+    char* cb;
+    const int64_t* d_totals;
+    if ((rc = stage_locally(x, part, in_cols, n_cols, n_rows, pc, conv_bytes, &cb, &d_totals))) return rc;
     if (T > 1) {
-        NCCL_TRY(n->AllGather(job.d_totals, x->d_counts, N, ncclInt64, x->comm, s), "ncclAllGather(counts)");
+        NCCL_TRY(n->AllGather(d_totals, x->d_counts, N, ncclInt64, x->comm, s), "ncclAllGather(counts)");
     } else {
-        CUDA_TRY(cudaMemcpyAsync(x->d_counts, job.d_totals, sizeof(int64_t) * N, cudaMemcpyDeviceToDevice, s), "copy counts");
+        CUDA_TRY(cudaMemcpyAsync(x->d_counts, d_totals, sizeof(int64_t) * N, cudaMemcpyDeviceToDevice, s), "copy counts");
     }
     CUDA_TRY(cudaMemcpyAsync(x->h_counts, x->d_counts, sizeof(int64_t) * (size_t)N * T, cudaMemcpyDeviceToHost, s), "D2H counts");
     // sender-side conversions + per-destination byte counts of the string columns
     std::vector<int> var_cols;
     for (int i = 0; i < n_cols; ++i) {
-        const XCol& c0 = xc[i];
-        if (c0.in_valid && (rc = launch_bits_to_bytes((const uint8_t*)(sb + c0.st_valid), 0, n_rows, (uint8_t*)(sb + c0.cv_valid), s))) return rc;
-        if (c0.has_valid && !c0.in_valid && n_rows > 0)  // no nulls among my rows: all-valid lane
-            CUDA_TRY(cudaMemsetAsync(sb + c0.cv_valid, 1, (size_t)n_rows, s), "memset");
-        if (c0.kind == DFD_COL_BOOL && (rc = launch_bits_to_bytes((const uint8_t*)(sb + c0.st_values), 0, n_rows, (uint8_t*)(sb + c0.cv_values), s))) return rc;
-        if (c0.kind >= DFD_COL_UTF8) {
-            if ((rc = launch_offsets_to_lengths(sb + c0.st_off, c0.ow, n_rows, sb + c0.cv_len, s))) return rc;
-            int64_t* d_meta = (int64_t*)(sb + meta_off) + (size_t)var_cols.size() * 2 * N;
-            if ((rc = launch_var_dest_bytes(sb + c0.st_off, c0.ow, part->d_part_starts, N, d_meta, d_meta + N, s))) return rc;
+        const PushCol& q = pc[i];
+        uint8_t* send_valid = (uint8_t*)(cb + cv[i].send_valid);
+        if (q.in_valid && (rc = launch_bits_to_bytes((const uint8_t*)q.validity, 0, n_rows, send_valid, s))) return rc;
+        if (q.nullable && !q.in_valid && n_rows > 0)  // no nulls among my rows: all-valid lane
+            CUDA_TRY(cudaMemsetAsync(send_valid, 1, (size_t)n_rows, s), "memset");
+        if (q.kind == DFD_COL_BOOL && (rc = launch_bits_to_bytes((const uint8_t*)q.values, 0, n_rows, (uint8_t*)(cb + cv[i].send_values), s))) return rc;
+        if (q.var_index >= 0) {
+            if ((rc = launch_offsets_to_lengths(q.offsets, q.ow, n_rows, cb + cv[i].send_values, s))) return rc;
+            int64_t* d_meta = (int64_t*)(cb + meta_off) + (size_t)q.var_index * 2 * N;
+            if ((rc = launch_var_dest_bytes(q.offsets, q.ow, part->d_part_starts, N, d_meta, d_meta + N, s))) return rc;
             var_cols.push_back(i);
         }
     }
     // byte-count matrices of the string columns: all-gather [T][N] per column
-    const size_t V = var_cols.size();
     std::vector<int64_t> h_first(V * N), h_bytes(V * (size_t)T * N);
     int64_t* d_bytes_all = nullptr;
     if (V) {
         if ((rc = x->bytes_all.ensure(sizeof(int64_t) * V * (size_t)T * N + 256, c->device))) return rc;
         d_bytes_all = (int64_t*)x->bytes_all.ptr;
         for (size_t v = 0; v < V; ++v) {
-            int64_t* d_meta = (int64_t*)(sb + meta_off) + v * 2 * N;
+            int64_t* d_meta = (int64_t*)(cb + meta_off) + v * 2 * N;
             if (T > 1) {
                 ncclResult_t r = n->AllGather(d_meta, d_bytes_all + v * (size_t)T * N, N, ncclInt64, x->comm, s);
                 if (r != ncclSuccess) return nccl_error(r, "ncclAllGather(byte counts)");
@@ -1246,88 +1252,62 @@ int dfd_shuffle_device(dfd_exchange* x, dfd_partitioner* part, int mode, const d
             return set_error(DFD_ERR_CAPACITY, "column %d: receives %lld string bytes but out values_bytes is %lld", var_cols[v],
                              (long long)total, (long long)out_cols[var_cols[v]].values_bytes);
     }
-    // receiver temporaries: u8-per-row images of bitmaps, lengths of strings
     size_t rtmp = 0;
     for (int i = 0; i < n_cols; ++i) {
-        XCol& c0 = xc[i];
-        if (c0.has_valid) { c0.rv_valid = rtmp; rtmp += al((size_t)recv_rows + 64); }
-        if (c0.kind == DFD_COL_BOOL) { c0.rv_values = rtmp; rtmp += al((size_t)recv_rows + 64); }
-        if (c0.kind >= DFD_COL_UTF8) { c0.rv_len = rtmp; rtmp += al((size_t)(recv_rows + 1) * c0.ow + 64); }
+        const PushCol& q = pc[i];
+        if (q.nullable) { cv[i].recv_valid = rtmp; rtmp += al((size_t)recv_rows + 64); }
+        if (q.kind != DFD_COL_FIXED) { cv[i].recv_values = rtmp; rtmp += al((size_t)(recv_rows + 1) * lane_width(q) + 64); }
     }
     const size_t rsums = rtmp;
     rtmp += al((size_t)(recv_rows / (256 * 8) + 4) * 8);
     if ((rc = x->recv_tmp.ensure(rtmp + 256, c->device))) return rc;
     char* rt = (char*)x->recv_tmp.ptr;
-    const int64_t* cnt = x->h_counts;
-    // one "lane" = one fixed-stride row stream to move with the row count matrix
-    struct Lane { const char* src; char* dst; size_t w; };
+    // one "lane" = one stream of w-byte units with its own T x N count matrix, send starts [N] and receive starts [P][T]:
+    // the row lanes, then the bytes of every string column
+    struct Lane { const char* src; char* dst; size_t w; const int64_t* cnt; const int64_t* send; const int64_t* recv; };
     std::vector<Lane> lanes;
+    auto row_lane = [&](const char* src, char* dst, size_t w) { lanes.push_back({src, dst, w, x->h_counts, send_start.data(), recv_start.data()}); };
     for (int i = 0; i < n_cols; ++i) {
-        const XCol& c0 = xc[i];
-        if (c0.kind == DFD_COL_FIXED) lanes.push_back({sb + c0.st_values, (char*)out_cols[i].values, (size_t)c0.width});
-        if (c0.kind == DFD_COL_BOOL) lanes.push_back({sb + c0.cv_values, rt + c0.rv_values, 1});
-        if (c0.kind >= DFD_COL_UTF8) lanes.push_back({sb + c0.cv_len, rt + c0.rv_len, (size_t)c0.ow});
-        if (c0.has_valid) lanes.push_back({sb + c0.cv_valid, rt + c0.rv_valid, 1});
+        const PushCol& q = pc[i];
+        if (q.kind == DFD_COL_FIXED) row_lane(q.values, (char*)out_cols[i].values, (size_t)q.width);
+        else row_lane(cb + cv[i].send_values, rt + cv[i].recv_values, lane_width(q));
+        if (q.nullable) row_lane(cb + cv[i].send_valid, rt + cv[i].recv_valid, 1);
     }
+    for (size_t v = 0; v < V; ++v)
+        lanes.push_back({pc[var_cols[v]].values, (char*)out_cols[var_cols[v]].values, 1, h_bytes.data() + v * (size_t)T * N, h_first.data() + v * N,
+                         brecv_start[v].data()});
     if (T > 1) NCCL_TRY(n->GroupStart(), "ncclGroupStart");
     for (const Lane& ln : lanes) {
-        for (uint32_t g = 0; g < N; ++g) {  // my rows of destination g -> its owner
+        for (uint32_t g = 0; g < N; ++g) {  // my units of destination g -> its owner
             const int peer = (int)(g / P);
-            const int64_t rows = cnt[(int64_t)x->rank * N + g];
-            if (rows == 0) continue;
+            const int64_t units = ln.cnt[(int64_t)x->rank * N + g];
+            if (units == 0) continue;
             if (peer == x->rank) {
-                CUDA_TRY(cudaMemcpyAsync(ln.dst + (size_t)recv_start[(size_t)(g % P) * T + x->rank] * ln.w, ln.src + (size_t)send_start[g] * ln.w,
-                                         (size_t)rows * ln.w, cudaMemcpyDeviceToDevice, s), "local segment copy");
+                CUDA_TRY(cudaMemcpyAsync(ln.dst + (size_t)ln.recv[(size_t)(g % P) * T + x->rank] * ln.w, ln.src + (size_t)ln.send[g] * ln.w,
+                                         (size_t)units * ln.w, cudaMemcpyDeviceToDevice, s), "local segment copy");
             } else {
-                NCCL_TRY(n->Send(ln.src + (size_t)send_start[g] * ln.w, (size_t)rows * ln.w, ncclInt8, peer, x->comm, s), "ncclSend");
-                x->bytes_sent += (uint64_t)rows * ln.w;
+                NCCL_TRY(n->Send(ln.src + (size_t)ln.send[g] * ln.w, (size_t)units * ln.w, ncclInt8, peer, x->comm, s), "ncclSend");
+                x->bytes_sent += (uint64_t)units * ln.w;
             }
         }
-        for (int r = 0; r < T; ++r) {  // every producer's rows of my P destinations
+        for (int r = 0; r < T; ++r) {  // every producer's units of my P destinations
             if (r == x->rank) continue;
             for (uint32_t q = 0; q < P; ++q) {
-                const int64_t rows = cnt[(int64_t)r * N + (int64_t)x->rank * P + q];
-                if (rows == 0) continue;
-                NCCL_TRY(n->Recv(ln.dst + (size_t)recv_start[(size_t)q * T + r] * ln.w, (size_t)rows * ln.w, ncclInt8, r, x->comm, s), "ncclRecv");
-                x->bytes_received += (uint64_t)rows * ln.w;
-            }
-        }
-    }
-    for (size_t v = 0; v < V; ++v) {  // string bytes, with their own count matrix
-        const int i = var_cols[v];
-        const int64_t* bc = h_bytes.data() + v * (size_t)T * N;
-        const char* src = sb + xc[i].st_values;
-        char* dst = (char*)out_cols[i].values;
-        for (uint32_t g = 0; g < N; ++g) {
-            const int peer = (int)(g / P);
-            const int64_t nb = bc[(int64_t)x->rank * N + g];
-            if (nb == 0) continue;
-            if (peer == x->rank) {
-                CUDA_TRY(cudaMemcpyAsync(dst + brecv_start[v][(size_t)(g % P) * T + x->rank], src + h_first[v * N + g], (size_t)nb,
-                                         cudaMemcpyDeviceToDevice, s), "local bytes copy");
-            } else {
-                NCCL_TRY(n->Send(src + h_first[v * N + g], (size_t)nb, ncclInt8, peer, x->comm, s), "ncclSend(bytes)");
-                x->bytes_sent += (uint64_t)nb;
-            }
-        }
-        for (int r = 0; r < T; ++r) {
-            if (r == x->rank) continue;
-            for (uint32_t q = 0; q < P; ++q) {
-                const int64_t nb = bc[(int64_t)r * N + (int64_t)x->rank * P + q];
-                if (nb == 0) continue;
-                NCCL_TRY(n->Recv(dst + brecv_start[v][(size_t)q * T + r], (size_t)nb, ncclInt8, r, x->comm, s), "ncclRecv(bytes)");
-                x->bytes_received += (uint64_t)nb;
+                const int64_t units = ln.cnt[(int64_t)r * N + (int64_t)x->rank * P + q];
+                if (units == 0) continue;
+                NCCL_TRY(n->Recv(ln.dst + (size_t)ln.recv[(size_t)q * T + r] * ln.w, (size_t)units * ln.w, ncclInt8, r, x->comm, s), "ncclRecv");
+                x->bytes_received += (uint64_t)units * ln.w;
             }
         }
     }
     if (T > 1) NCCL_TRY(n->GroupEnd(), "ncclGroupEnd");
     // receiver-side rebuild of bitmaps and offsets
     for (int i = 0; i < n_cols; ++i) {
-        const XCol& c0 = xc[i];
-        if (c0.has_valid && (rc = launch_bytes_to_bits((const uint8_t*)(rt + c0.rv_valid), recv_rows, out_cols[i].validity, s))) return rc;
-        if (c0.kind == DFD_COL_BOOL && (rc = launch_bytes_to_bits((const uint8_t*)(rt + c0.rv_values), recv_rows, out_cols[i].values, s))) return rc;
-        if (c0.kind >= DFD_COL_UTF8 &&
-            (rc = launch_lengths_to_offsets(rt + c0.rv_len, c0.ow, recv_rows, (unsigned long long*)(rt + rsums), out_cols[i].offsets, s)))
+        const PushCol& q = pc[i];
+        if (q.nullable && (rc = launch_bytes_to_bits((const uint8_t*)(rt + cv[i].recv_valid), recv_rows, out_cols[i].validity, s))) return rc;
+        if (q.kind == DFD_COL_BOOL && (rc = launch_bytes_to_bits((const uint8_t*)(rt + cv[i].recv_values), recv_rows, out_cols[i].values, s))) return rc;
+        if (q.var_index >= 0 &&
+            (rc = launch_lengths_to_offsets(rt + cv[i].recv_values, q.ow, recv_rows, (unsigned long long*)(rt + rsums), out_cols[i].offsets, s)))
             return rc;
     }
     CUDA_TRY(cudaStreamSynchronize(s), "nccl exchange");
@@ -1346,18 +1326,16 @@ int dfd_shuffle_host(dfd_exchange* x, dfd_partitioner* part, const dfd_column* i
                      int64_t* chunk_part_starts) {
     if (!x || !part || !in_cols || !out_cols || !chunk_part_starts || n_chunks < 1 || n_rows < 0)
         return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_shuffle_host: bad arguments");
-    dfd_ctx* c = x->ctx;
     const uint32_t P = partitions_per_task;
-    if ((uint64_t)P * x->world != part->N)
-        return set_error(DFD_ERR_INVALID_ARGUMENT, "num_partitions %u != partitions_per_task %u x %d workers", part->N, P, x->world);
     for (int i = 0; i < n_cols; ++i)
         if (in_cols[i].kind != DFD_COL_FIXED || in_cols[i].validity || in_cols[i].offset != 0 || out_cols[i].kind != DFD_COL_FIXED ||
             out_cols[i].width != in_cols[i].width || !in_cols[i].values || !out_cols[i].values)
             return set_error(DFD_ERR_UNSUPPORTED, "column %d: dfd_shuffle_host moves fixed-width non-null columns", i);
-    std::lock_guard<std::mutex> lk(c->mu);
-    CUDA_TRY(cudaSetDevice(c->device), "cudaSetDevice");
-    int rc = ensure_count_buffers(x, part->N);
+    std::unique_lock<std::mutex> lk;
+    int rc = begin_shuffle(x, part, in_cols, out_cols, P, "dfd_shuffle_host", lk);
     if (rc) return rc;
+    x->shuffles += (uint64_t)n_chunks - 1;  // one collective fused shuffle per chunk
+    dfd_ctx* c = x->ctx;
     if (!x->s_h2d) {
         CUDA_TRY(cudaStreamCreateWithFlags(&x->s_h2d, cudaStreamNonBlocking), "stream");
         CUDA_TRY(cudaStreamCreateWithFlags(&x->s_d2h, cudaStreamNonBlocking), "stream");
@@ -1403,7 +1381,6 @@ int dfd_shuffle_host(dfd_exchange* x, dfd_partitioner* part, const dfd_column* i
         }
         CUDA_TRY(cudaStreamWaitEvent(c->stream, x->e_h2d[k], 0), "wait");
         if (i >= 2) CUDA_TRY(cudaStreamWaitEvent(c->stream, x->e_d2h[k], 0), "wait");  // my window slot k has been drained
-        x->shuffles++;
         if ((rc = fused_shuffle_locked(x, part, dev_in.data(), n_cols, rows, P, k, 2, win.data(), x->e_k[k]))) return rc;
         const int64_t got = x->h_my_starts[P];
         if (out_row + got > out_capacity_rows)
@@ -1430,16 +1407,9 @@ int dfd_shuffle_host(dfd_exchange* x, dfd_partitioner* part, const dfd_column* i
  * matters). */
 int dfd_shuffle_device_async(dfd_exchange* x, dfd_partitioner* part, const dfd_column* in_cols, int n_cols, int64_t n_rows,
                              uint32_t partitions_per_task, dfd_column* out_cols) {
-    if (!x || !part || !in_cols || !out_cols) return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_shuffle_device_async: NULL argument");
-    dfd_ctx* c = x->ctx;
-    if (part->ctx != c) return set_error(DFD_ERR_INVALID_ARGUMENT, "partitioner and exchange belong to different contexts");
-    if (partitions_per_task < 1 || (uint64_t)partitions_per_task * x->world != part->N)
-        return set_error(DFD_ERR_INVALID_ARGUMENT, "num_partitions %u != partitions_per_task %u x %d workers", part->N, partitions_per_task, x->world);
-    std::lock_guard<std::mutex> lk(c->mu);
-    CUDA_TRY(cudaSetDevice(c->device), "cudaSetDevice");
-    int rc = ensure_count_buffers(x, part->N);
+    std::unique_lock<std::mutex> lk;
+    int rc = begin_shuffle(x, part, in_cols, out_cols, partitions_per_task, "dfd_shuffle_device_async", lk);
     if (rc) return rc;
-    x->shuffles++;
     return fused_shuffle_locked(x, part, in_cols, n_cols, n_rows, partitions_per_task, 0, 1, out_cols, nullptr, /*sync=*/false);
 }
 
@@ -1448,10 +1418,12 @@ int dfd_exchange_wait(dfd_exchange* x, int64_t* part_starts_host) {
     dfd_ctx* c = x->ctx;
     std::lock_guard<std::mutex> lk(c->mu);
     CUDA_TRY(cudaSetDevice(c->device), "cudaSetDevice");
-    if (!x->pending_async) return set_error(DFD_ERR_INVALID_ARGUMENT, "no asynchronous shuffle is pending");
-    int rc = fused_shuffle_finish(x, x->pending_P);
+    dfd_exchange::Pending& pd = x->pending;
+    if (pd.kind != dfd_exchange::Pending::DENSE) return set_error(DFD_ERR_INVALID_ARGUMENT, "no asynchronous shuffle is pending");
+    pd.kind = dfd_exchange::Pending::NONE;
+    int rc = fused_shuffle_finish(x, pd.P, pd.row_bytes);
     if (rc) return rc;
-    if (part_starts_host) memcpy(part_starts_host, x->h_my_starts, sizeof(int64_t) * (x->pending_P + 1));
+    if (part_starts_host) memcpy(part_starts_host, x->h_my_starts, sizeof(int64_t) * (pd.P + 1));
     return DFD_OK;
 }
 
@@ -1459,97 +1431,80 @@ int dfd_exchange_wait(dfd_exchange* x, int64_t* part_starts_host) {
  * (dense layout) when the schema / partition count is outside the single-pass kernel's envelope. */
 int dfd_shuffle_device_onepass(dfd_exchange* x, dfd_partitioner* part, const dfd_column* in_cols, int n_cols, int64_t n_rows,
                                uint32_t partitions_per_task, dfd_column* out_cols) {
-    if (!x || !part || !in_cols || !out_cols) return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_shuffle_device_onepass: NULL argument");
-    dfd_ctx* c = x->ctx;
-    if (part->ctx != c) return set_error(DFD_ERR_INVALID_ARGUMENT, "partitioner and exchange belong to different contexts");
     const uint32_t P = partitions_per_task;
-    if (P < 1 || (uint64_t)P * x->world != part->N)
-        return set_error(DFD_ERR_INVALID_ARGUMENT, "num_partitions %u != partitions_per_task %u x %d workers", part->N, P, x->world);
-    std::lock_guard<std::mutex> lk(c->mu);
-    CUDA_TRY(cudaSetDevice(c->device), "cudaSetDevice");
-    int rc = ensure_count_buffers(x, part->N);
+    std::unique_lock<std::mutex> lk;
+    int rc = begin_shuffle(x, part, in_cols, out_cols, P, "dfd_shuffle_device_onepass", lk);
     if (rc) return rc;
-    x->shuffles++;
-    x->last_in.assign(in_cols, in_cols + n_cols);
-    x->last_part = part;
-    x->last_rows = n_rows;
-    x->pending_push = false;
-    if (!onepass_supported(x, part, in_cols, out_cols, n_cols, P)) {
-        // nullable / boolean / string columns (or > 256 partitions): the push transport moves every column kind
-        x->pending_onepass = false;
-        return push_shuffle_locked(x, part, in_cols, n_cols, n_rows, P, out_cols);
-    }
-    rc = onepass_shuffle_locked(x, part, in_cols, n_cols, n_rows, P, 0, 1, out_cols);
-    if (rc == DFD_OK) x->last_out.assign(out_cols, out_cols + n_cols);
-    return rc;
+    if (!onepass_supported(part, in_cols, out_cols, n_cols, P))  // nullable / boolean / string columns (or > 256 partitions):
+        return push_shuffle_locked(x, part, in_cols, n_cols, n_rows, P, out_cols);  // the push transport moves every column kind
+    return onepass_shuffle_locked(x, part, in_cols, n_cols, n_rows, P, 0, 1, out_cols);
 }
 
 /* Complete the last dfd_shuffle_device_onepass: per local partition q and producer r, rows
  * [seg_starts[q*T + r], +seg_counts[q*T + r]) of every out column.  If a sub-window overflowed on ANY worker
  * (every worker sees every producer's flag, so all take the same branch) the shuffle is re-run through the two-pass
  * fused path with exact counts; the segments then describe its dense layout. */
+// Segment q * T + r = producer r's counts[r * stride + q] rows of my partition q: back to back from x->h_my_starts[q] in the
+// dense layout (sub_cap 0), else at the start of its sub-window of sub_cap rows.  Returns the rows of all segments.
+static uint64_t fill_segments(const dfd_exchange* x, uint32_t P, const int64_t* counts, size_t stride, int64_t sub_cap, int64_t* seg_starts,
+                              int64_t* seg_counts) {
+    const int T = x->world;
+    uint64_t rows = 0;
+    for (uint32_t q = 0; q < P; ++q) {
+        int64_t run = sub_cap ? (int64_t)q * T * sub_cap : x->h_my_starts[q];
+        for (int r = 0; r < T; ++r) {
+            const int64_t cnt = counts[(size_t)r * stride + q];
+            if (seg_starts) seg_starts[(size_t)q * T + r] = run;
+            if (seg_counts) seg_counts[(size_t)q * T + r] = cnt;
+            run += sub_cap ? sub_cap : cnt;
+            rows += (uint64_t)cnt;
+        }
+    }
+    return rows;
+}
+
 int dfd_exchange_collect(dfd_exchange* x, dfd_column* out_cols, int64_t* seg_starts, int64_t* seg_counts) {
     if (!x) return set_error(DFD_ERR_INVALID_ARGUMENT, "NULL exchange");
     dfd_ctx* c = x->ctx;
     std::lock_guard<std::mutex> lk(c->mu);
     CUDA_TRY(cudaSetDevice(c->device), "cudaSetDevice");
     const int T = x->world;
-    const uint32_t P = x->pending_P;
-    if (x->pending_push) {  // the push transport completes inside the call: hand out its segments
-        for (size_t i = 0; i < x->push_seg_starts.size(); ++i) {
-            if (seg_starts) seg_starts[i] = x->push_seg_starts[i];
-            if (seg_counts) seg_counts[i] = x->push_seg_counts[i];
-        }
-        return DFD_OK;
-    }
-    if (!x->pending_onepass) {
-        if (!x->pending_async) return set_error(DFD_ERR_INVALID_ARGUMENT, "no shuffle is pending");
-        int rc = fused_shuffle_finish(x, P);  // dense two-pass layout: producers contiguous per partition
-        if (rc) return rc;
-        CUDA_TRY(cudaMemcpy(x->h_counts, x->d_counts, sizeof(int64_t) * (size_t)P * T * T, cudaMemcpyDeviceToHost), "D2H counts");
-        for (uint32_t q = 0; q < P; ++q) {
-            int64_t run = x->h_my_starts[q];
-            for (int r = 0; r < T; ++r) {
-                const int64_t cnt = x->h_counts[(size_t)r * P * T + (size_t)x->rank * P + q];
-                if (seg_starts) seg_starts[(size_t)q * T + r] = run;
-                if (seg_counts) seg_counts[(size_t)q * T + r] = cnt;
-                run += cnt;
+    dfd_exchange::Pending& pd = x->pending;
+    const uint32_t P = pd.P;
+    int rc;
+    switch (pd.kind) {
+        case dfd_exchange::Pending::SEGMENTS:  // the push transport completes inside the call: hand out its segments
+            for (size_t i = 0; i < pd.seg_starts.size(); ++i) {
+                if (seg_starts) seg_starts[i] = pd.seg_starts[i];
+                if (seg_counts) seg_counts[i] = pd.seg_counts[i];
             }
-        }
-        return DFD_OK;
+            return DFD_OK;
+        case dfd_exchange::Pending::DENSE:  // dense two-pass layout: producers contiguous per partition
+            pd.kind = dfd_exchange::Pending::NONE;
+            if ((rc = fused_shuffle_finish(x, P, pd.row_bytes))) return rc;
+            CUDA_TRY(cudaMemcpy(x->h_counts, x->d_counts, sizeof(int64_t) * (size_t)P * T * T, cudaMemcpyDeviceToHost), "D2H counts");
+            fill_segments(x, P, x->h_counts + (size_t)x->rank * P, (size_t)P * T, 0, seg_starts, seg_counts);
+            return DFD_OK;
+        case dfd_exchange::Pending::REGIONS:
+            break;
+        default:
+            return set_error(DFD_ERR_INVALID_ARGUMENT, "no shuffle is pending");
     }
     CUDA_TRY(cudaStreamSynchronize(c->stream), "single-pass shuffle");
-    x->pending_onepass = false;
+    pd.kind = dfd_exchange::Pending::NONE;
     if (x->h_seg_flags[MAX_RANKS]) return set_error(DFD_ERR_INTERNAL, "a peer worker never signalled completion of the shuffle (did it fail?)");
     bool overflow = false;
     for (int r = 0; r < T; ++r) overflow |= x->h_seg_flags[r] != 0;
     if (overflow) {
         // exact re-run: counts all-gather -> plan -> two-pass peer scatter (every worker takes this branch)
         x->onepass_fallbacks++;
-        std::vector<dfd_column> outs(x->last_in.size());
-        int rc = fused_shuffle_locked(x, x->last_part, x->last_in.data(), (int)x->last_in.size(), x->last_rows, P, 0, 1, outs.data(), nullptr, /*sync=*/true);
-        if (rc) return rc;
+        std::vector<dfd_column> outs(pd.in.size());
+        if ((rc = fused_shuffle_locked(x, pd.part, pd.in.data(), (int)pd.in.size(), pd.rows, P, 0, 1, outs.data(), nullptr, /*sync=*/true))) return rc;
         if (out_cols) for (size_t i = 0; i < outs.size(); ++i) out_cols[i] = outs[i];
-        for (uint32_t q = 0; q < P; ++q) {
-            int64_t run = x->h_my_starts[q];
-            for (int r = 0; r < T; ++r) {
-                const int64_t cnt = x->h_seg_counts[(size_t)r * P + q];
-                if (seg_starts) seg_starts[(size_t)q * T + r] = run;
-                if (seg_counts) seg_counts[(size_t)q * T + r] = cnt;
-                run += cnt;
-            }
-        }
+        fill_segments(x, P, x->h_seg_counts, P, 0, seg_starts, seg_counts);
         return DFD_OK;
     }
-    uint64_t rows = 0;
-    for (uint32_t q = 0; q < P; ++q)
-        for (int r = 0; r < T; ++r) {
-            const int64_t cnt = x->h_seg_counts[(size_t)r * P + q];
-            if (seg_starts) seg_starts[(size_t)q * T + r] = ((int64_t)q * T + r) * x->pending_sub_cap;
-            if (seg_counts) seg_counts[(size_t)q * T + r] = cnt;
-            rows += (uint64_t)cnt;
-        }
-    x->bytes_received += rows * x->pending_row_bytes;
+    x->bytes_received += fill_segments(x, P, x->h_seg_counts, P, pd.sub_cap, seg_starts, seg_counts) * pd.row_bytes;
     return DFD_OK;
 }
 
@@ -1574,6 +1529,7 @@ struct dfd_shuffle_stream {
 int dfd_shuffle_stream_begin(dfd_exchange* x, dfd_partitioner* part, const dfd_column* in_cols, int n_cols, int64_t n_rows,
                              uint32_t partitions_per_task, const uint8_t* nullable, dfd_shuffle_stream** out) {
     if (!x || !part || !in_cols || !out || n_rows < 0 || n_cols < 1) return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_shuffle_stream_begin: bad arguments");
+    if (part->ctx != x->ctx) return set_error(DFD_ERR_INVALID_ARGUMENT, "partitioner and exchange belong to different contexts");
     if (partitions_per_task < 1 || (uint64_t)partitions_per_task * x->world != part->N)
         return set_error(DFD_ERR_INVALID_ARGUMENT, "num_partitions %u != partitions_per_task %u x %d workers", part->N, partitions_per_task, x->world);
     dfd_shuffle_stream* st = new (std::nothrow) dfd_shuffle_stream();
@@ -1678,25 +1634,15 @@ int dfd_exchange_gather(dfd_exchange* x, int route, const dfd_column* in_cols, i
     const uint32_t n_slices = route == DFD_ROUTE_SHUFFLE ? P * (uint32_t)x->world : P;
     dfd_ctx* c = x->ctx;
     std::lock_guard<std::mutex> lk(c->mu);
+    x->pending.kind = dfd_exchange::Pending::NONE;
     CUDA_TRY(cudaSetDevice(c->device), "cudaSetDevice");
     if (!x->window_ready) return set_error(DFD_ERR_INVALID_ARGUMENT, "the exchange needs dfd_exchange_setup_window first");
     cudaStream_t s = c->stream;
-    std::vector<PushCol> pc(n_cols);
-    int V = 0;
-    for (int i = 0; i < n_cols; ++i) {
-        const dfd_column& ic = in_cols[i];
-        PushCol& q = pc[i];
-        q = PushCol{};
-        q.kind = ic.kind; q.width = ic.width; q.ow = ic.kind == DFD_COL_LARGE_UTF8 ? 8 : 4; q.var_index = -1;
-        if (ic.kind == DFD_COL_UTF8 || ic.kind == DFD_COL_LARGE_UTF8 || ic.kind == DFD_COL_BINARY) q.var_index = V++;
-        else if (ic.kind != DFD_COL_FIXED && ic.kind != DFD_COL_BOOL) return set_error(DFD_ERR_UNSUPPORTED, "column %d: unknown column kind %d", i, ic.kind);
-        q.in_valid = ic.validity != nullptr;
-        q.nullable = out_cols[i].validity != nullptr || q.in_valid;
-        q.values = (const char*)ic.values; q.offsets = (const char*)ic.offsets; q.validity = (const char*)ic.validity; q.offset = ic.offset;
-    }
+    std::vector<PushCol> pc;
+    int rc = describe_columns(in_cols, out_cols, n_cols, pc);
+    if (rc) return rc;
     // device copy of the slice boundaries + scratch for the per-slice byte offsets
-    const size_t need = ((size_t)(n_slices + 1) * 8 + 255) / 256 * 256 + (size_t)(V + 1) * n_slices * 8 + 256;
-    int rc;
+    const size_t need = ((size_t)(n_slices + 1) * 8 + 255) / 256 * 256 + (size_t)(n_var_cols(pc) + 1) * n_slices * 8 + 256;
     if ((rc = x->recv_tmp.ensure(need, c->device))) return rc;
     int64_t* d_starts = (int64_t*)x->recv_tmp.ptr;
     char* scratch = (char*)x->recv_tmp.ptr + ((size_t)(n_slices + 1) * 8 + 255) / 256 * 256;
@@ -1706,11 +1652,12 @@ int dfd_exchange_gather(dfd_exchange* x, int route, const dfd_column* in_cols, i
     CUDA_TRY(cudaStreamSynchronize(s), "sync");  // (slice_starts is caller memory)
     Route R{route, P, x->world, consumer_tasks};
     x->shuffles++;
-    x->pending_P = P;
     return push_slices_locked(x, pc, in_cols, R, d_starts, scratch, out_cols);
 }
 
-uint32_t dfd_exchange_pending_segments(const dfd_exchange* x) { return x && x->pending_push ? (uint32_t)x->push_seg_starts.size() : 0; }
+uint32_t dfd_exchange_pending_segments(const dfd_exchange* x) {
+    return x && x->pending.kind == dfd_exchange::Pending::SEGMENTS ? (uint32_t)x->pending.seg_starts.size() : 0;
+}
 
 int dfd_exchange_stats(dfd_exchange* x, uint64_t* bytes_sent, uint64_t* bytes_received, uint64_t* shuffles) {
     if (!x) return set_error(DFD_ERR_INVALID_ARGUMENT, "NULL exchange");

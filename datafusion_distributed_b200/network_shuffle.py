@@ -65,6 +65,21 @@ def nccl_unique_id() -> bytes:
     return bytes(buf)
 
 
+def _nullable_outs(in_cols: Sequence[DeviceColumn], nullable: Optional[Sequence[bool]]):
+    """Output descriptors that carry the schema's nullable flag of every column (`nullable[i]`; default: the columns of
+    this worker that have a validity bitmap), as the segment exchanges expect them on entry."""
+    c_out = (nv.DfdColumn * len(in_cols))()
+    for i, c in enumerate(in_cols):
+        if (nullable[i] if nullable is not None else bool(c.validity)):
+            c_out[i].validity = 1  # (flag only: the library replaces it with the bitmap's address)
+    return c_out
+
+
+def _window_columns(c_out, types, exchange: "ShuffleExchange", length: int = 0) -> List[DeviceColumn]:
+    """DeviceColumns over the buffers the library set in `c_out` (they live in `exchange`'s receive window)."""
+    return [DeviceColumn(c.kind, c.width, c.values or 0, c.offsets or 0, c.validity or 0, 0, length, exchange, t) for c, t in zip(c_out, types)]
+
+
 class ShuffleExchange:
     """One worker's endpoint of the exchange (≙ WorkerConnectionPool + the worker's
     ExecuteTask server, src/worker/worker_connection_pool.rs:60-113)."""
@@ -131,15 +146,18 @@ class NetworkShuffleExec:
         return self.input_stage.plan
 
     # -- data plane --------------------------------------------------------------
+    def _partitioner(self, exchange: ShuffleExchange):
+        """Handle of the producers' Hash(keys, P x task_count) partitioner, created on first use."""
+        if self._part is None:
+            self._part = HashPartitioner(exchange.ctx, self.input_stage.plan)
+        return self._part._h
+
     def shuffle(self, exchange: ShuffleExchange, in_cols: Sequence[DeviceColumn], n_rows: int, mode: int = nv.EXCHANGE_FUSED,
                 out_cols: Optional[List[DeviceColumn]] = None, out_capacity_rows: int = 0):
         """Run the collective for this worker: as producer task `rank` it contributes `in_cols`,
         as consumer task `rank` it receives its P partitions."""
         if len(self.input_stage.tasks) != exchange.world or self.task_count != exchange.world:
             raise ValueError("this exchange runs one producer and one consumer task per GPU worker")
-        ctx = exchange.ctx
-        if self._part is None:
-            self._part = HashPartitioner(ctx, self.input_stage.plan)
         P = self.properties.partition_count
         c_in = columns_to_c(in_cols)
         if mode == nv.EXCHANGE_NCCL:
@@ -149,22 +167,19 @@ class NetworkShuffleExec:
         else:
             c_out = (nv.DfdColumn * len(in_cols))()
         starts = (C.c_int64 * (P + 1))()
-        nv.check(nv.lib().dfd_shuffle_device(exchange._h, self._part._h, mode, c_in, len(in_cols), n_rows, P, c_out,
+        nv.check(nv.lib().dfd_shuffle_device(exchange._h, self._partitioner(exchange), mode, c_in, len(in_cols), n_rows, P, c_out,
                                              out_capacity_rows, starts))
         if mode == nv.EXCHANGE_FUSED:
-            out_cols = [DeviceColumn(c_out[i].kind, c_out[i].width, c_out[i].values or 0, 0, 0, 0, int(starts[P]), exchange,
-                                     in_cols[i].arrow_type) for i in range(len(in_cols))]
+            out_cols = _window_columns(c_out, [c.arrow_type for c in in_cols], exchange, int(starts[P]))
         self._out = list(out_cols)
         self._starts = np.frombuffer(starts, dtype=np.int64).copy()
         return self._out, self._starts
 
     def shuffle_async(self, exchange: ShuffleExchange, in_cols: Sequence[DeviceColumn], n_rows: int):
         """Fused shuffle enqueued on the worker's stream without a host sync (`dfd_shuffle_device_async`)."""
-        if self._part is None:
-            self._part = HashPartitioner(exchange.ctx, self.input_stage.plan)
         P = self.properties.partition_count
         c_out = (nv.DfdColumn * len(in_cols))()
-        nv.check(nv.lib().dfd_shuffle_device_async(exchange._h, self._part._h, columns_to_c(in_cols), len(in_cols), n_rows, P, c_out))
+        nv.check(nv.lib().dfd_shuffle_device_async(exchange._h, self._partitioner(exchange), columns_to_c(in_cols), len(in_cols), n_rows, P, c_out))
         self._pending = (c_out, [c.arrow_type for c in in_cols], exchange)
 
     def wait(self, exchange: ShuffleExchange):
@@ -173,8 +188,7 @@ class NetworkShuffleExec:
         starts = (C.c_int64 * (P + 1))()
         nv.check(nv.lib().dfd_exchange_wait(exchange._h, starts))
         c_out, types, _ = self._pending
-        self._out = [DeviceColumn(c_out[i].kind, c_out[i].width, c_out[i].values or 0, 0, 0, 0, int(starts[P]), exchange, types[i])
-                     for i in range(len(types))]
+        self._out = _window_columns(c_out, types, exchange, int(starts[P]))
         self._starts = np.frombuffer(starts, dtype=np.int64).copy()
         return self._out, self._starts
 
@@ -187,14 +201,9 @@ class NetworkShuffleExec:
         carry a validity bitmap).  Complete it with `collect()`."""
         if len(self.input_stage.tasks) != exchange.world or self.task_count != exchange.world:
             raise ValueError("this exchange runs one producer and one consumer task per GPU worker")
-        if self._part is None:
-            self._part = HashPartitioner(exchange.ctx, self.input_stage.plan)
         P = self.properties.partition_count
-        c_out = (nv.DfdColumn * len(in_cols))()
-        for i, c in enumerate(in_cols):
-            if (nullable[i] if nullable is not None else bool(c.validity)):
-                c_out[i].validity = 1  # (flag only: the library replaces it with the bitmap's address)
-        nv.check(nv.lib().dfd_shuffle_device_onepass(exchange._h, self._part._h, columns_to_c(in_cols), len(in_cols), n_rows, P, c_out))
+        c_out = _nullable_outs(in_cols, nullable)
+        nv.check(nv.lib().dfd_shuffle_device_onepass(exchange._h, self._partitioner(exchange), columns_to_c(in_cols), len(in_cols), n_rows, P, c_out))
         self._pending = (c_out, [c.arrow_type for c in in_cols], exchange)
 
     @staticmethod
@@ -243,8 +252,7 @@ class NetworkShuffleExec:
         nv.check(nv.lib().dfd_exchange_collect(exchange._h, c_out, starts, counts))
         self._seg_starts = np.frombuffer(starts, dtype=np.int64).reshape(P, T).copy()
         self._seg_counts = np.frombuffer(counts, dtype=np.int64).reshape(P, T).copy()
-        self._out = [DeviceColumn(c_out[i].kind, c_out[i].width, c_out[i].values or 0, c_out[i].offsets or 0, c_out[i].validity or 0, 0, 0,
-                                  exchange, types[i]) for i in range(len(types))]
+        self._out = _window_columns(c_out, types, exchange)
         self._starts = None
         return self._out, self._seg_starts, self._seg_counts
 
@@ -265,10 +273,7 @@ class NetworkShuffleExec:
         (out columns, seg_starts[P][T], seg_counts[P][T])."""
         P, T = self.properties.partition_count, exchange.world
         starts = (C.c_int64 * (P * T + 1))(*[int(v) for v in part_starts])
-        c_out = (nv.DfdColumn * len(in_cols))()
-        for i, c in enumerate(in_cols):
-            if (nullable[i] if nullable is not None else bool(c.validity)):
-                c_out[i].validity = 1
+        c_out = _nullable_outs(in_cols, nullable)
         nv.check(nv.lib().dfd_exchange_gather(exchange._h, nv.ROUTE_SHUFFLE, columns_to_c(in_cols), len(in_cols), starts, P, T, c_out))
         self._pending = (c_out, [c.arrow_type for c in in_cols], exchange)
         return self.collect(exchange)
@@ -278,12 +283,10 @@ class NetworkShuffleExec:
         """Back-pressured shuffle (`dfd_shuffle_stream_*`): a generator of rounds (out columns, seg_starts[P][T],
         seg_counts[P][T]); a round's buffers are valid until the next one is requested.  Rounds shrink automatically
         when a consumer's receive window cannot hold one (skew / small windows) instead of failing."""
-        if self._part is None:
-            self._part = HashPartitioner(exchange.ctx, self.input_stage.plan)
         P, T = self.properties.partition_count, exchange.world
         h = C.c_void_p()
         nl = (C.c_uint8 * len(in_cols))(*[1 if (nullable[i] if nullable is not None else bool(c.validity)) else 0 for i, c in enumerate(in_cols)])
-        nv.check(nv.lib().dfd_shuffle_stream_begin(exchange._h, self._part._h, columns_to_c(in_cols), len(in_cols), n_rows, P, nl, C.byref(h)))
+        nv.check(nv.lib().dfd_shuffle_stream_begin(exchange._h, self._partitioner(exchange), columns_to_c(in_cols), len(in_cols), n_rows, P, nl, C.byref(h)))
         try:
             while True:
                 c_out = (nv.DfdColumn * len(in_cols))()
@@ -291,8 +294,7 @@ class NetworkShuffleExec:
                 nv.check(nv.lib().dfd_shuffle_stream_next(h, c_out, starts, counts, C.byref(done)))
                 if done.value:
                     break
-                outs = [DeviceColumn(c_out[i].kind, c_out[i].width, c_out[i].values or 0, c_out[i].offsets or 0, c_out[i].validity or 0, 0, 0,
-                                     exchange, in_cols[i].arrow_type) for i in range(len(in_cols))]
+                outs = _window_columns(c_out, [c.arrow_type for c in in_cols], exchange)
                 yield outs, np.frombuffer(starts, dtype=np.int64).reshape(P, T).copy(), np.frombuffer(counts, dtype=np.int64).reshape(P, T).copy()
             r, sp = C.c_uint64(), C.c_uint64()
             nv.lib().dfd_shuffle_stream_stats(h, C.byref(r), C.byref(sp))
@@ -304,11 +306,9 @@ class NetworkShuffleExec:
                      host_out: Sequence[DeviceColumn], out_capacity_rows: int) -> np.ndarray:
         """Host-to-host pipelined shuffle (`dfd_shuffle_host`): `host_in` / `host_out` describe HOST (pinned)
         column buffers.  Returns chunk_part_starts[n_chunks][P+1] (absolute row offsets into host_out)."""
-        if self._part is None:
-            self._part = HashPartitioner(exchange.ctx, self.input_stage.plan)
         P = self.properties.partition_count
         starts = (C.c_int64 * (n_chunks * (P + 1)))()
-        nv.check(nv.lib().dfd_shuffle_host(exchange._h, self._part._h, columns_to_c(host_in), len(host_in), n_rows, P, n_chunks,
+        nv.check(nv.lib().dfd_shuffle_host(exchange._h, self._partitioner(exchange), columns_to_c(host_in), len(host_in), n_rows, P, n_chunks,
                                            columns_to_c(host_out), out_capacity_rows, starts))
         return np.frombuffer(starts, dtype=np.int64).reshape(n_chunks, P + 1).copy()
 
@@ -352,18 +352,14 @@ class _GatherExec:
             raise ValueError("one producer task per GPU worker")
         P = self.partitions
         starts = (C.c_int64 * (P + 1))(*[int(v) for v in slice_starts])
-        c_out = (nv.DfdColumn * len(in_cols))()
-        for i, c in enumerate(in_cols):
-            if (nullable[i] if nullable is not None else bool(c.validity)):
-                c_out[i].validity = 1
+        c_out = _nullable_outs(in_cols, nullable)
         nv.check(nv.lib().dfd_exchange_gather(exchange._h, self.ROUTE, columns_to_c(in_cols), len(in_cols), starts, P, self.task_count, c_out))
         n = nv.lib().dfd_exchange_pending_segments(exchange._h)
         ss, sc = (C.c_int64 * max(n, 1))(), (C.c_int64 * max(n, 1))()
         nv.check(nv.lib().dfd_exchange_collect(exchange._h, c_out, ss, sc))
         self._starts = np.frombuffer(ss, dtype=np.int64)[:n].copy()
         self._counts = np.frombuffer(sc, dtype=np.int64)[:n].copy()
-        self._out = [DeviceColumn(c_out[i].kind, c_out[i].width, c_out[i].values or 0, c_out[i].offsets or 0, c_out[i].validity or 0, 0, 0,
-                                  exchange, in_cols[i].arrow_type) for i in range(len(in_cols))]
+        self._out = _window_columns(c_out, [c.arrow_type for c in in_cols], exchange)
         return self._out, self._starts, self._counts
 
 

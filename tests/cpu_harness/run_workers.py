@@ -4,7 +4,7 @@ push transport and compare every (partition, producer) segment with the single-n
 
     python run_workers.py <harness.so> <world> <scenario> [seed]
 
-scenario: shuffle | stream | coalesce | broadcast | mismatch | onepass | onepass_overflow | host | peer_missing | mixed | nccl | fused"""
+scenario: shuffle | stream | coalesce | broadcast | mismatch | onepass | onepass_overflow | host | peer_missing | mixed | nccl | fused | stale"""
 import ctypes as C
 import os
 import sys
@@ -270,6 +270,45 @@ def worker(lib, rank, world, uid, scenario, seed, errors, barrier):
             one_single_pass(seed + 3)
             one_single_pass(seed + 4)
             one_push(seed + 5)
+        elif scenario == "stale":
+            # collect reports the LAST shuffle only: a push result is dropped as soon as another shuffle starts, an asynchronous
+            # two-pass shuffle is completed by collect in its dense layout, and after an NCCL-mode shuffle (complete inside the
+            # call) nothing is pending
+            tabs = [fixed_table(r, 800 + 5 * r, seed, False) for r in range(world)]
+            kp = []
+            cols_ = to_columns(tabs[rank], kp)
+            n_c, n_r = tabs[rank].num_columns, tabs[rank].num_rows
+            p1 = VP()
+            check(lib, lib.dfd_partitioner_create(ctx, N, (C.c_int32 * 1)(0), 1, None, C.byref(p1)), "dfd_partitioner_create")
+            d_ = [orc.partition_ids([t.column("key")], t.num_rows, N) for t in tabs]
+            one_push(seed + 1)
+            o_ = (COL * n_c)()
+            check(lib, lib.dfd_shuffle_device_async(ex, p1, cols_, n_c, n_r, P, o_), "dfd_shuffle_device_async")
+            assert lib.dfd_exchange_pending_segments(ex) == 0
+            st_, ct_ = (C.c_int64 * (P * world))(), (C.c_int64 * (P * world))()
+            check(lib, lib.dfd_exchange_collect(ex, o_, st_, ct_), "dfd_exchange_collect")
+            for sgm in range(P * world):
+                r, q = sgm % world, sgm // world
+                want = tabs[r].take(pa.array(np.nonzero(d_[r] == rank * P + q)[0]))
+                assert int(ct_[sgm]) == want.num_rows, ("stale", rank, sgm, int(ct_[sgm]), want.num_rows)
+                if sgm + 1 < P * world:  # dense: every segment starts where the one before it ends
+                    assert st_[sgm + 1] == st_[sgm] + ct_[sgm], ("stale", rank, sgm)
+                for c, f in enumerate(tabs[rank].schema):
+                    assert segment_to_arrow(o_[c], f, int(st_[sgm]), int(ct_[sgm])).equals(want.column(c).combine_chunks()), ("stale", rank, sgm, f.name)
+            barrier.wait()
+            one_push(seed + 2)
+            cap = sum(t.num_rows for t in tabs) + 8
+            bufs = [np.zeros(cap * 8 + 64, dtype=np.uint8) for _ in range(n_c)]
+            o_ = (COL * n_c)()
+            for i, b in enumerate(bufs):
+                o_[i].kind, o_[i].width, o_[i].values = cols_[i].kind, cols_[i].width, b.ctypes.data
+            ps = (C.c_int64 * (P + 1))()
+            check(lib, lib.dfd_shuffle_device(ex, p1, 0, cols_, n_c, n_r, P, o_, cap, ps), "dfd_shuffle_device(NCCL)")
+            assert lib.dfd_exchange_pending_segments(ex) == 0
+            rc = lib.dfd_exchange_collect(ex, o_, st_, ct_)
+            assert rc == 1 and b"no shuffle is pending" in lib.dfd_last_error(), (rc, lib.dfd_last_error())
+            barrier.wait()
+            lib.dfd_partitioner_destroy(p1)
         elif scenario == "peer_missing":
             # the last worker fails before the exchange (it never enters the collective): the others must come back with an error
             # after the bounded flag wait — never hang (the coordinator then cancels the stage, impl_execute_task.rs:138-155)

@@ -111,6 +111,11 @@ def test_transports_alternate_on_one_window(exchange_harness, world):
     run(exchange_harness, world, "mixed")
 
 
+@pytest.mark.parametrize("world", [1, 2])
+def test_collect_reports_only_the_last_shuffle(exchange_harness, world):
+    run(exchange_harness, world, "stale")
+
+
 def test_a_missing_peer_is_an_error_after_a_bounded_wait_not_a_hang(exchange_harness):
     run(exchange_harness, 3, "peer_missing", HARNESS_FLAG_TIMEOUT_MS="400")
 
