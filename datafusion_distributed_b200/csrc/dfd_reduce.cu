@@ -11,7 +11,7 @@
 //   k_group_count    groups per destination partition (representatives only)      -> exclusive scan (host, N+1 values)
 //   k_group_place    every group gets an output row inside its partition; key columns copied, states initialised
 //   k_group_combine  every input row folds its states into its group's output row with atomics
-//                    (SUM i64 / f64 / i128 (two 64-bit adds with carry), MIN / MAX i64 / f64)
+//                    (SUM i64 / f64 / i128 (two 64-bit adds with carry), MIN / MAX i64, MIN / MAX f64 under totalOrder)
 // Integer / byte work; random access into an L2-resident table for the cardinalities PartialReduce is used for.
 #include <cuda_runtime.h>
 
@@ -124,14 +124,15 @@ __global__ void __launch_bounds__(256) k_group_count(const __grid_constant__ Red
     }
 }
 
-__device__ __forceinline__ void state_init(const ReduceCol& c, char* dst) {
+// `rep` = the group's representative row.  Float MIN / MAX start from its value, not from +-inf: an all-NaN group then
+// yields one of its own NaNs, and folding the representative in again in k_group_combine changes nothing.
+__device__ __forceinline__ void state_init(const ReduceCol& c, char* dst, int64_t rep) {
     switch (c.op) {
         case DFD_AGG_SUM_I64: case DFD_AGG_SUM_F64: *(uint64_t*)dst = 0; break;
         case DFD_AGG_SUM_I128: ((uint64_t*)dst)[0] = 0; ((uint64_t*)dst)[1] = 0; break;
         case DFD_AGG_MIN_I64: *(long long*)dst = 0x7fffffffffffffffLL; break;
         case DFD_AGG_MAX_I64: *(long long*)dst = (long long)0x8000000000000000ULL; break;
-        case DFD_AGG_MIN_F64: *(double*)dst = __longlong_as_double(0x7ff0000000000000LL); break;   // +inf
-        case DFD_AGG_MAX_F64: *(double*)dst = __longlong_as_double((long long)0xfff0000000000000ULL); break;  // -inf
+        case DFD_AGG_MIN_F64: case DFD_AGG_MAX_F64: *(uint64_t*)dst = *(const uint64_t*)(c.in + rep * 8); break;
     }
 }
 
@@ -149,26 +150,24 @@ __global__ void __launch_bounds__(256) k_group_place(const __grid_constant__ Red
                 const char* src = col.in + (int64_t)rep * col.width;
                 for (int b = 0; b < col.width; ++b) dst[b] = src[b];
             } else {
-                state_init(col, dst);
+                state_init(col, dst, (int64_t)rep);
             }
         }
     }
 }
 
-__device__ __forceinline__ void atomic_min_f64(double* addr, double v) {
-    unsigned long long* a = (unsigned long long*)addr;
-    unsigned long long old = *a;
-    while (v < __longlong_as_double((long long)old)) {
-        const unsigned long long prev = atomicCAS(a, old, (unsigned long long)__double_as_longlong(v));
-        if (prev == old) break;
-        old = prev;
-    }
+// IEEE 754 totalOrder as a signed integer: flipping the magnitude bits of negative values makes the int64 order
+// -NaN < -inf < ... < -0.0 < +0.0 < ... < +inf < +NaN, with NaNs ordered by payload.  Only identical bits tie, so the
+// merged MIN / MAX is the same whatever order the rows arrive in.
+__device__ __forceinline__ long long f64_total_order_key(unsigned long long bits) {
+    return (long long)(bits ^ ((unsigned long long)((long long)bits >> 63) >> 1));
 }
-__device__ __forceinline__ void atomic_max_f64(double* addr, double v) {
-    unsigned long long* a = (unsigned long long*)addr;
+template <bool MAX>
+__device__ __forceinline__ void atomic_minmax_f64(unsigned long long* a, unsigned long long v) {
+    const long long vk = f64_total_order_key(v);
     unsigned long long old = *a;
-    while (v > __longlong_as_double((long long)old)) {
-        const unsigned long long prev = atomicCAS(a, old, (unsigned long long)__double_as_longlong(v));
+    while (MAX ? vk > f64_total_order_key(old) : vk < f64_total_order_key(old)) {
+        const unsigned long long prev = atomicCAS(a, old, v);
         if (prev == old) break;
         old = prev;
     }
@@ -187,8 +186,8 @@ __global__ void __launch_bounds__(256) k_group_combine(const __grid_constant__ R
                 case DFD_AGG_SUM_F64: atomicAdd((double*)dst, *(const double*)src); break;
                 case DFD_AGG_MIN_I64: atomicMin((long long*)dst, *(const long long*)src); break;
                 case DFD_AGG_MAX_I64: atomicMax((long long*)dst, *(const long long*)src); break;
-                case DFD_AGG_MIN_F64: atomic_min_f64((double*)dst, *(const double*)src); break;
-                case DFD_AGG_MAX_F64: atomic_max_f64((double*)dst, *(const double*)src); break;
+                case DFD_AGG_MIN_F64: atomic_minmax_f64<false>((unsigned long long*)dst, *(const unsigned long long*)src); break;
+                case DFD_AGG_MAX_F64: atomic_minmax_f64<true>((unsigned long long*)dst, *(const unsigned long long*)src); break;
                 case DFD_AGG_SUM_I128: {
                     // two's complement 128-bit add as two 64-bit atomics: each add propagates its OWN carry exactly once
                     const unsigned long long lo = ((const unsigned long long*)src)[0], hi = ((const unsigned long long*)src)[1];

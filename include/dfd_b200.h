@@ -431,7 +431,11 @@ int dfd_exchange_phase_ms(dfd_exchange* x, double* out3, uint64_t* n_shuffles);
  * per distinct key, partition p = rows [out_part_starts[p], out_part_starts[p+1]) of out_cols (capacity n_rows; row order
  * inside a partition is unspecified, like a hash aggregate's).  Feed it to dfd_exchange_gather(DFD_ROUTE_SHUFFLE) — the
  * rows never leave the GPU between Partial aggregation, repartition, PartialReduce and the exchange.
- * Fixed-width non-null keys and states (nullable group keys / states: DFD_ERR_UNSUPPORTED).  Synchronous. */
+ * Fixed-width non-null keys and states (nullable group keys / states: DFD_ERR_UNSUPPORTED).  Synchronous.
+ * Integer SUMs wrap (two's complement, mod 2^64 / 2^128).  Float SUM is the IEEE sum in an unspecified order.  Float
+ * MIN / MAX order values by IEEE 754 totalOrder (Rust's f64::total_cmp): -NaN < -inf < ... < -0.0 < +0.0 < ... < +inf
+ * < +NaN, NaNs ordered by payload.  So a +NaN wins MAX and a -NaN wins MIN, -0.0 is below +0.0, an all-NaN group yields
+ * one of its NaNs, and the result's bits are one input row's bits, the same on every run. */
 typedef enum {
     DFD_AGG_SUM_I64 = 0,  /* also COUNT states */
     DFD_AGG_SUM_F64 = 1,

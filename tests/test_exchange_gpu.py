@@ -19,9 +19,19 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 @pytest.mark.parametrize("mode", [nv.EXCHANGE_NCCL, nv.EXCHANGE_FUSED])
 def test_single_worker_shuffle_equals_local_repartition(ctx, mode):
+    check_single_worker_shuffle(ctx, mode, 8)
+
+
+@pytest.mark.parametrize("P", [16, 17, 48])
+def test_single_worker_fused_shuffle_past_the_aligned_cutoff(ctx, P):
+    """Peer kernels write out aligned runs up to 16 partitions; past that their plain (KV == K) instantiations run."""
+    check_single_worker_shuffle(ctx, nv.EXCHANGE_FUSED, P)
+
+
+def check_single_worker_shuffle(ctx, mode, P):
     import pyarrow as pa
 
-    n, P = 300_007, 8
+    n = 300_007
     cols = cfg2_columns(n, 4)
     ex = dfd.ShuffleExchange(ctx, 0, 1, None)
     ex.setup_window(n * 4 * 8 + (1 << 20))
@@ -45,11 +55,21 @@ def test_single_worker_shuffle_equals_local_repartition(ctx, mode):
 
 
 def test_single_worker_onepass_shuffle_segments(ctx):
+    check_single_worker_onepass_shuffle(ctx, 8)
+
+
+@pytest.mark.parametrize("P", [16, 17, 48, 256])
+def test_single_worker_onepass_shuffle_past_the_aligned_cutoff(ctx, P):
+    """The single-pass peer kernel's aligned write-out ends at 16 partitions; 256 is the single-pass maximum."""
+    check_single_worker_onepass_shuffle(ctx, P)
+
+
+def check_single_worker_onepass_shuffle(ctx, P):
     """Single-pass fused exchange at world=1: partition q is one segment (one producer), bit-exact and in input order;
     back-to-back shuffles reuse the window (ready/done flags)."""
     import pyarrow as pa
 
-    n, P = 300_007, 8
+    n = 300_007
     cols = cfg2_columns(n, 4)
     ex = dfd.ShuffleExchange(ctx, 0, 1, None)
     ex.setup_window(int(n * 4 * 8 * 1.5) + (1 << 20))
@@ -85,6 +105,35 @@ def test_single_worker_onepass_shuffle_segments(ctx):
         assert np.array_equal(got, ref[1][rs[q]:rs[q + 1]])
     ex.close()
     ex2.close()
+
+
+def test_single_worker_onepass_shuffle_every_cta_handles_many_tiles(ctx):
+    """Single-pass peer kernel at world=1 with every CTA looping over several tiles, 4 / 8 / 16-byte columns.  They are
+    fixed-width and non-null: a nullable, boolean or string column would send the shuffle to the push transport."""
+    import pyarrow as pa
+
+    from tests.util import expected_partitions, multi_tile_rows
+
+    n, P = multi_tile_rows(), 48
+    rng = np.random.Generator(np.random.PCG64(21))
+    key = rng.integers(-(2**63), 2**63 - 1, n, dtype=np.int64, endpoint=True)
+    raw = rng.integers(0, 255, n * 16, dtype=np.uint8).tobytes()
+    arrays = [pa.array(key), pa.array(rng.integers(-(2**31), 2**31 - 1, n, dtype=np.int32)), pa.array(np.arange(n, dtype=np.int64)),
+              pa.Array.from_buffers(pa.decimal128(38, 0), n, [None, pa.py_buffer(raw)])]
+    ex = dfd.ShuffleExchange(ctx, 0, 1, None)
+    ex.setup_window(int(n * 36 * 1.5) + (1 << 20))
+    node = dfd.NetworkShuffleExec.try_new(dfd.Partitioning.Hash([0], P), uuid.uuid4(), 1, 1, 1)
+    node.shuffle_onepass(ex, [dfd.DeviceColumn.from_arrow(ctx, a) for a in arrays], n)
+    outs, seg_starts, seg_counts = node.collect(ex)
+    assert nv.lib().dfd_exchange_onepass_fallbacks(ex._h) == 0
+    order, ref_starts = expected_partitions(orc.partition_ids([key], n, P), P)
+    assert np.array_equal(seg_counts[:, 0], np.diff(ref_starts))
+    for q in range(P):
+        idx = pa.array(order[ref_starts[q]:ref_starts[q + 1]])
+        for c, arr in enumerate(arrays):
+            got = dfd.NetworkShuffleExec.segment_to_arrow(ctx, outs[c], int(seg_starts[q, 0]), int(seg_counts[q, 0]))
+            assert got.equals(arr.take(idx)), (q, c)
+    ex.close()
 
 
 def test_fused_window_overflow_is_reported(ctx):

@@ -9,7 +9,7 @@ import pytest
 
 import datafusion_distributed_b200 as dfd
 from oracle import oracle as orc
-from tests.util import cfg2_columns, expected_partitions
+from tests.util import cfg2_columns, edge_sizes, expected_partitions, multi_tile_rows, tile_geometry
 
 pytestmark = pytest.mark.gpu
 
@@ -37,7 +37,7 @@ def check_against_oracle(ctx, arrays, key_cols, N, region_rows=None):
     return part, starts, counts
 
 
-@pytest.mark.parametrize("n_rows", [0, 1, 31, 32, 33, 1535, 1536, 1537, 3072, 100_003])
+@pytest.mark.parametrize("n_rows", edge_sizes())
 def test_onepass_ragged_sizes(ctx, n_rows):
     check_against_oracle(ctx, cfg2_columns(n_rows, 3), [0], 8)
 
@@ -77,6 +77,80 @@ def test_onepass_mixed_widths_nulls_bools(ctx):
     arrays = [key, c8, c16, c32, f64, bl, dec]
     for N in (8, 48):
         check_against_oracle(ctx, arrays, [0, 3], N)
+
+
+def mixed_table(n, seed):
+    """Nullable Int64 and Int32 keys, UInt8 / Int16 / Float64 / Decimal128 payload and a nullable Boolean."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    key = pa.array(rng.integers(0, 1 << 40, n, dtype=np.int64), mask=rng.random(n) < 0.5)
+    c8 = pa.array(rng.integers(0, 255, n, dtype=np.uint8))
+    c16 = pa.array(rng.integers(-30000, 30000, n, dtype=np.int16))
+    c32 = pa.array(rng.integers(0, 1 << 31, n, dtype=np.int32), mask=rng.random(n) < 0.5)
+    f64 = pa.array(rng.standard_normal(n))
+    bl = pa.array(rng.random(n) < 0.5, mask=rng.random(n) < 0.3)
+    dec = pa.Array.from_buffers(pa.decimal128(38, 0), n, [None, pa.py_buffer(rng.integers(0, 255, n * 16, dtype=np.uint8).tobytes())])
+    return [key, c8, c16, c32, f64, bl, dec]
+
+
+def test_onepass_every_cta_handles_many_tiles_mixed_schema(ctx):
+    """Generic two-column key, 1 / 2 / 4 / 8 / 16-byte columns (the 16-byte one split into row ranges), nulls and a
+    boolean column (follow-up launches), with every CTA looping over several tiles."""
+    check_against_oracle(ctx, mixed_table(multi_tile_rows(), 31), [0, 3], 48)
+
+
+def test_onepass_every_cta_handles_many_tiles_cfg2_two_keys(ctx):
+    check_against_oracle(ctx, cfg2_columns(multi_tile_rows(), 4), [0, 1], 8)
+
+
+def sliced_payload(n, offset, seed):
+    """Payload columns of widths 1, 2, 4, 8 and 16 and a nullable Boolean, each a slice at `offset` of a longer array:
+    the source of every column tile is then off its 16-byte alignment (or, for offset 1 and width 1, its byte count)."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    m = n + offset + 5
+    arrays = [pa.array(rng.integers(0, 255, m, dtype=np.uint8)), pa.array(rng.integers(-30000, 30000, m, dtype=np.int16)),
+              pa.array(rng.integers(-(1 << 31), 1 << 31, m, dtype=np.int32), mask=rng.random(m) < 0.2),
+              pa.array(rng.integers(-(1 << 62), 1 << 62, m, dtype=np.int64)),
+              pa.Array.from_buffers(pa.decimal128(38, 0), m, [None, pa.py_buffer(rng.integers(0, 255, m * 16, dtype=np.uint8).tobytes())]),
+              pa.array(rng.random(m) < 0.5, mask=rng.random(m) < 0.3)]
+    return [a.slice(offset, n) for a in arrays]
+
+
+@pytest.mark.parametrize("offset", [1, 3, 13])
+@pytest.mark.parametrize("sliced_key", [False, True])
+def test_onepass_and_two_pass_sliced_inputs(ctx, offset, sliced_key):
+    """Sliced payload (Arrow offset 1 / 3 / 13) under an unsliced non-null Int64 key, where the single-pass producer
+    takes the fast key path and only its element-wise fallback copy changes, and under a sliced key (generic key path).
+    The same inputs go through the two-pass partition()."""
+    n, N = 3 * tile_geometry()[1] * 7 + 11, 12
+    rng = np.random.Generator(np.random.PCG64(offset))
+    key = pa.array(rng.integers(-(1 << 63), (1 << 63) - 1, n + offset, dtype=np.int64))
+    key = key.slice(offset, n) if sliced_key else key.slice(0, n)
+    arrays = [key] + sliced_payload(n, offset, 40 + offset)
+    check_against_oracle(ctx, arrays, [0], N)
+    part = dfd.HashPartitioner(ctx, dfd.Partitioning.Hash([0], N))
+    outs, starts = part.partition(dev_cols(ctx, arrays), n)
+    order, ref_starts = expected_partitions(orc.partition_ids([key], n, N), N)
+    assert np.array_equal(starts, ref_starts)
+    idx = pa.array(order)
+    for c, arr in enumerate(arrays):
+        assert outs[c].to_arrow(ctx, 0, n).equals(arr.take(idx)), (c, arr.type)
+
+
+def test_onepass_region_capacity_exactly_max_count(ctx):
+    """Regions of exactly the largest destination's row count fit without a re-run; one row less re-runs exactly once
+    into the dense layout, bit-exact."""
+    n, N = 200_003, 8
+    cols = cfg2_columns(n, 3)
+    c = np.bincount(orc.partition_ids([cols[0]], n, N), minlength=N)
+    mx = int(c.max())
+    assert (mx - 1) * N >= n  # one row less still holds every row in total: valid input
+    before = ctx.metrics()["onepass_reruns"]
+    _, starts, counts = check_against_oracle(ctx, cols, [0], N, region_rows=mx)
+    assert ctx.metrics()["onepass_reruns"] == before
+    assert np.array_equal(starts, np.arange(N) * mx)
+    _, starts, counts = check_against_oracle(ctx, cols, [0], N, region_rows=mx - 1)
+    assert ctx.metrics()["onepass_reruns"] == before + 1
+    assert np.array_equal(starts[1:], np.cumsum(counts)[:-1]) and starts[0] == 0  # dense after the re-run
 
 
 def test_onepass_many_columns_multiple_launches(ctx):

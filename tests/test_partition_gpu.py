@@ -12,7 +12,7 @@ import pytest
 
 import datafusion_distributed_b200 as dfd
 from oracle import oracle as orc
-from tests.util import cfg2_columns, expected_partitions, golden
+from tests.util import cfg2_columns, edge_sizes, expected_partitions, golden
 
 pytestmark = pytest.mark.gpu
 
@@ -112,7 +112,7 @@ def run_partition(ctx, arrays, key_cols, N):
     return outs, starts
 
 
-@pytest.mark.parametrize("n_rows", [0, 1, 31, 32, 33, 2047, 2048, 2049, 100_003])
+@pytest.mark.parametrize("n_rows", edge_sizes())
 def test_scatter_matches_oracle_ragged_sizes(ctx, n_rows):
     cols = cfg2_columns(n_rows, 3)
     outs, starts = run_partition(ctx, cols, [0], 8)
@@ -283,6 +283,38 @@ def test_scatter_variable_width_payload_and_keys(ctx, N):
         for c, arr in enumerate(arrays):
             got = outs[c].to_arrow(ctx, int(starts[p]), int(starts[p + 1]))
             assert got.equals(arr.take(idx)), (N, p, c)
+
+
+def _long_binary(rng, n):
+    """Binary values of 0 to 3000 bytes, most of them 256 to 1100 (the byte copy's long-value branch), about 5% null.
+    Lengths are random, so a long value's source and destination offsets agree mod 8 for some values and not others."""
+    lens = np.where(rng.random(n) < 0.7, rng.integers(256, 1101, n), rng.integers(0, 3001, n))
+    blob = rng.integers(32, 127, int(lens.sum()), dtype=np.uint8).tobytes()  # (printable ASCII: valid UTF-8 too)
+    ends = np.cumsum(lens)
+    null = rng.random(n) < 0.05
+    return pa.array([None if null[i] else blob[ends[i] - lens[i]:ends[i]] for i in range(n)], type=pa.binary())
+
+
+@pytest.mark.parametrize("N", [8, 48])
+def test_scatter_long_variable_width_values_as_keys_and_payload(ctx, N):
+    """Utf8 / LargeUtf8 / Binary values up to 3000 bytes, whole and sliced, as the hash keys (long-string hashing loops
+    many times) and as the payload they move with."""
+    rng = np.random.Generator(np.random.PCG64(N))
+    n = 6_007
+    bn = _long_binary(rng, n)
+    s = pa.Array.from_buffers(pa.string(), n, _long_binary(rng, n).buffers(), null_count=-1)
+    ls = _long_binary(rng, n).cast(pa.string()).cast(pa.large_string())
+    idx_col = pa.array(np.arange(n, dtype=np.int32))
+    for arrays in ([s, ls, bn, idx_col], [a.slice(7, n - 20) for a in (s, ls, bn, idx_col)]):
+        m = len(arrays[0])
+        outs, starts = run_partition(ctx, arrays, [0, 1, 2], N)
+        order, ref_starts = expected_partitions(orc.partition_ids(arrays[:3], m, N), N)
+        assert np.array_equal(starts, ref_starts)
+        for p in range(N):
+            idx = pa.array(order[starts[p]:starts[p + 1]])
+            for c, arr in enumerate(arrays):
+                got = outs[c].to_arrow(ctx, int(starts[p]), int(starts[p + 1]))
+                assert got.equals(arr.take(idx)), (N, m, p, c)
 
 
 def test_variable_width_sliced_input_and_empty(ctx):
