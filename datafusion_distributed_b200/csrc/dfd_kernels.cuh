@@ -679,11 +679,12 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src, uint32
 struct OnePassSmem {
     uint32_t off_bars, off_tix, off_delta, off_ob, off_wc, off_ts, off_scan, off_misc, off_vs, off_src, off_d8, total;
 };
-template <int THREADS, int K, int NB>
+// S: ring items per column of a tile (each one a range of T / S rows), so a slot holds T * width / S bytes
+template <int THREADS, int K, int NB, int S>
 __host__ __device__ __forceinline__ OnePassSmem onepass_smem_layout(uint32_t N, uint32_t width, bool peer, bool aligned) {
     constexpr uint32_t T = THREADS * K, W = THREADS / 32;
     OnePassSmem L;
-    const uint32_t slot_bytes = (T * width + 127u) & ~127u;  // ring of NB input tiles first (128-B aligned bulk-copy destinations)
+    const uint32_t slot_bytes = (T / S * width + 127u) & ~127u;  // ring of NB sub-tile items first (128-B aligned bulk-copy destinations)
     L.off_bars = NB * slot_bytes;                             // full[NB] | empty[NB]
     L.off_tix = L.off_bars + 2u * NB * 8u;                    // tile of the header item in each slot (int64)
     L.off_delta = L.off_tix + NB * 8u;
@@ -699,14 +700,72 @@ __host__ __device__ __forceinline__ OnePassSmem onepass_smem_layout(uint32_t N, 
     return L;
 }
 
+// Phase clocks of k_scatter_onepass, compiled in only with -DDFD_ONEPASS_CLOCKS (scripts/onepass_clocks.py): clock64()
+// cycles per phase, summed over every CTA as seen by consumer thread 0 and by the producer's lane 0.
+enum OnePassClock {
+    CLK_WAIT_HEADER,    // consumer: FULL waits on the key-tile (header) items
+    CLK_WAIT_KEYCOL,    // consumer: FULL waits on the payload items that re-read the key column
+    CLK_WAIT_COL,       // consumer: FULL waits on the other payload items
+    CLK_PHASE1,         // consumer: hash + rank + counts + permutation (after the header wait)
+    CLK_LOOKBACK,       // consumer: decoupled look-back, spin included
+    CLK_SCATTER,        // consumer: scatter of all columns, FULL waits included
+    CLK_PROD_WAIT,      // producer: EMPTY waits
+    CLK_CONSUMER_TOTAL, // consumer: whole kernel
+    CLK_PRODUCER_TOTAL, // producer: whole kernel
+    CLK_TILES,          // tiles (count, not cycles)
+    CLK_COUNT
+};
+#ifdef DFD_ONEPASS_CLOCKS
+static __device__ unsigned long long g_onepass_clocks[CLK_COUNT];
+#define DFD_CLK_START(v) const long long v = clock64()
+#define DFD_CLK_ADD(on, i, v) \
+    do { if (on) atomicAdd(g_onepass_clocks + (i), (unsigned long long)(clock64() - (v))); } while (0)
+#define DFD_CLK_COUNT(on, i) \
+    do { if (on) atomicAdd(g_onepass_clocks + (i), 1ull); } while (0)
+#else
+#define DFD_CLK_START(v) ((void)0)
+#define DFD_CLK_ADD(on, i, v) ((void)0)
+#define DFD_CLK_COUNT(on, i) ((void)0)
+#endif
+
+// Calls f(E{}, split) with the element type E of a cw-byte column in a ring of sizeof(V)-byte elements; split: the column
+// arrives as `parts` items of consecutive row ranges (S > 1, or a 16-byte column in an 8-byte ring) rather than one.
+template <typename V, int S, typename F>
+__device__ __forceinline__ void onepass_by_width(int cw, int parts, F&& f) {
+    if constexpr (S > 1) {
+        switch (cw) {
+            case 16: if constexpr (sizeof(V) >= 8) f(uint4{}, std::true_type{}); break;
+            case 8: if constexpr (sizeof(V) >= 8) f((unsigned long long)0, std::true_type{}); break;
+            case 4: if constexpr (sizeof(V) >= 4) f((unsigned)0, std::true_type{}); break;
+            case 2: if constexpr (sizeof(V) >= 2) f((unsigned short)0, std::true_type{}); break;
+            default: f((unsigned char)0, std::true_type{}); break;
+        }
+    } else if (parts > 1) {
+        if constexpr (sizeof(V) == 8) f(uint4{}, std::true_type{});  // (the host only sends 16-byte columns this way)
+    } else {
+        switch (cw) {
+            case 16: if constexpr (sizeof(V) >= 16) f(uint4{}, std::false_type{}); break;
+            case 8: if constexpr (sizeof(V) >= 8) f((unsigned long long)0, std::false_type{}); break;
+            case 4: if constexpr (sizeof(V) >= 4) f((unsigned)0, std::false_type{}); break;
+            case 2: if constexpr (sizeof(V) >= 2) f((unsigned short)0, std::false_type{}); break;
+            default: f((unsigned char)0, std::false_type{}); break;
+        }
+    }
+}
+
 // ---------------------------------------------------------------------------
 // K2', single pass: no K1/K1b; every row is hashed once and every column read once.
 //
 // Warp-specialised persistent kernel (one CTA per resident slot): THREADS consumer threads + one producer warp.
-//  * producer warp: draws tile tickets (atomic, launch order) and streams, per tile, a header item (the key
-//    tile when the key is a single non-null 8-byte column) and one item per payload column into a ring of NB
-//    shared-memory slots with TMA bulk copies; per-slot full/empty mbarriers — loads run NB-1 items ahead of
-//    their use and never occupy registers.
+//  * producer warp: draws tile tickets (atomic, launch order) and streams, per tile, a header (the key tile
+//    when the key is a single non-null 8-byte column) and every payload column into a ring of NB shared-memory
+//    slots with TMA bulk copies; per-slot full/empty mbarriers — loads run NB-1 items ahead of their use and
+//    never occupy registers.  Every column of a tile (the header too) arrives as S items of T / S consecutive
+//    rows (2S for 16-byte columns in an 8-byte ring), so for the same shared memory a larger S means more,
+//    smaller items: the producer refills a slot as soon as its sub-tile is scattered and keeps up to NB-1
+//    of them in flight through phase 1 and the look-back.  Phase 1 holds all S header items at once: NB > S.
+//    (On H100 at cfg-2, S > 1 measures slower — each sub-item costs the consumers a pass of partial stores over
+//    all their slots — so the default is S = 1; DESIGN.md 4.1.)
 //  * consumers, per tile:
 //      phase 1 (on the header item of the NEXT tile): hash -> destination -> stable rank (ballot peers +
 //        per-warp counters); the tile's per-destination counts are published as look-back aggregates and
@@ -720,17 +779,20 @@ __host__ __device__ __forceinline__ OnePassSmem onepass_smem_layout(uint32_t N, 
 // region_stride); a tile that would overflow a region sets overflow_out and writes nothing — the counts stay
 // exact and the host re-runs with exact regions.
 // ---------------------------------------------------------------------------
-template <int THREADS, int K, int KV, int NB, int MIN_CTAS, bool FAST_I64, typename V, bool PEER>
+template <int THREADS, int K, int KV, int NB, int S, int MIN_CTAS, bool FAST_I64, typename V, bool PEER>
 __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(const __grid_constant__ ScatterParams P) {
     constexpr int T = THREADS * K;
     constexpr int W = THREADS / 32;
     constexpr int BAR = 1;  // named barrier of the consumer warps
     constexpr bool ROWS = (KV == K) && !PEER;
     static_assert(!std::is_same<V, BitColumn>::value, "bit columns take the two-pass kernel");
+    static_assert(NB > S, "phase 1 holds the S header items of a tile while the ring must still advance");
+    static_assert(W % S == 0, "each consumer warp's rows must lie in one header item");
+    constexpr int HROWS = T / S;  // rows of one header item
     extern __shared__ __align__(128) unsigned char smem[];
     const uint32_t N = P.N;
-    const OnePassSmem L = onepass_smem_layout<THREADS, K, NB>(N, (uint32_t)sizeof(V), PEER, KV != K);
-    const uint32_t slot_bytes = ((uint32_t)T * (uint32_t)sizeof(V) + 127u) & ~127u;
+    const OnePassSmem L = onepass_smem_layout<THREADS, K, NB, S>(N, (uint32_t)sizeof(V), PEER, KV != K);
+    const uint32_t slot_bytes = ((uint32_t)(T / S) * (uint32_t)sizeof(V) + 127u) & ~127u;
     unsigned long long* const FULL = (unsigned long long*)(smem + L.off_bars);
     unsigned long long* const EMPTY = FULL + NB;
     long long* const TIX = (long long*)(smem + L.off_tix);
@@ -749,10 +811,13 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
     if (w == W) {
         // =========================== producer warp ===========================
         const unsigned long long pol = l2_policy_evict_first();
+        DFD_CLK_START(clk_total);
         uint32_t seq = 0;
         auto acquire_slot = [&]() -> int {
             const int slot = (int)(seq % NB);
+            DFD_CLK_START(clk);
             if (lane == 0) mbar_wait(EMPTY + slot, ((seq / NB) & 1u) ^ 1u);
+            DFD_CLK_ADD(lane == 0, CLK_PROD_WAIT, clk);
             __syncwarp();
             return slot;
         };
@@ -782,17 +847,23 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
             t = __shfl_sync(0xffffffffu, t, 0);
             return (int64_t)t < P.n_tiles ? (int64_t)t : -1;
         };
+        // the header of a tile: S items, the first one carrying the tile number (-1: end of stream)
         auto emit_header = [&](int64_t tile) {
-            const int slot = acquire_slot();
-            if (lane == 0) TIX[slot] = tile;
-            if (FAST_I64 && tile >= 0) {
-                const int64_t row0 = tile * T;
-                const int rows = (int)((P.n_rows - row0) < T ? (P.n_rows - row0) : T);
-                fill(slot, P.keys.col[0].values, row0, rows, 8, false);  // key tile: default L2 policy (re-read as a payload column)
-            } else {
-                __syncwarp();
-                if (lane == 0) mbar_arrive(FULL + slot);
-                ++seq;
+            const int64_t row0 = tile * T;
+            const int rows = (int)((P.n_rows - row0) < T ? (P.n_rows - row0) : T);
+#pragma unroll 1
+            for (int h = 0; h < S; ++h) {
+                const int slot = acquire_slot();
+                if (h == 0 && lane == 0) TIX[slot] = tile;
+                const int rr = rows - h * HROWS;
+                if (FAST_I64 && tile >= 0 && rr > 0) {
+                    // key tile: default L2 policy (re-read as a payload column)
+                    fill(slot, P.keys.col[0].values, row0 + h * HROWS, rr < HROWS ? rr : HROWS, 8, false);
+                } else {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(FULL + slot);
+                    ++seq;
+                }
             }
         };
         int64_t cur = draw();
@@ -803,11 +874,11 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
             const int64_t row0 = cur * T;
             const int rows = (int)((P.n_rows - row0) < T ? (P.n_rows - row0) : T);
             for (int c = 0; c < P.n_cols; ++c) {
-                // a column wider than the ring's element type (16-byte values in an 8-byte ring) arrives as width / sizeof(V)
-                // items of T * sizeof(V) bytes each: consecutive ROW RANGES of the tile — the ring slots stay small enough for
-                // 4 resident CTAs whatever the schema
+                // every column arrives as S items of consecutive ROW RANGES of the tile; a column wider than the ring's element
+                // type (16-byte values in an 8-byte ring) as S * width / sizeof(V) of them — the ring slots stay the same size
+                // whatever the schema
                 const uint32_t cw = (uint32_t)P.cols[c].width;
-                const int parts = cw > (uint32_t)sizeof(V) ? (int)(cw / (uint32_t)sizeof(V)) : 1;
+                const int parts = (cw > (uint32_t)sizeof(V) ? (int)(cw / (uint32_t)sizeof(V)) : 1) * S;
                 const int rows_per = T / parts;
                 for (int h = 0; h < parts; ++h) {
                     const int slot = acquire_slot();
@@ -824,6 +895,7 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
             }
             cur = nxt;
         }
+        DFD_CLK_ADD(lane == 0, CLK_PRODUCER_TOTAL, clk_total);
         return;
     }
 
@@ -836,10 +908,14 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
     const int t0 = w * (K * 32) + lane;  // this thread's first tile-relative row; rows t0 + 32*j
     if (PEER)
         for (uint32_t p = threadIdx.x; p < N; p += THREADS) OUT_BASE[p] = P.peer_base[p / P.parts_per_rank];
+    [[maybe_unused]] const bool clk_on = threadIdx.x == 0;  // (phase clocks only)
+    DFD_CLK_START(clk_total);
     uint32_t cseq = 0;
-    auto wait_item = [&]() -> int {
-        const int slot = (int)(cseq % NB);
-        mbar_wait(FULL + slot, (cseq / NB) & 1u);
+    // ring slot of the item `ahead` items after the next one, once it has landed
+    auto wait_item = [&](uint32_t ahead = 0) -> int {
+        const uint32_t s = cseq + ahead;
+        const int slot = (int)(s % NB);
+        mbar_wait(FULL + slot, (s / NB) & 1u);
         return slot;
     };
     auto release_item = [&](int slot) {
@@ -847,15 +923,27 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
         if (lane == 0) mbar_arrive(EMPTY + slot);
         ++cseq;
     };
+    // the S header items of a tile, in order
+    auto release_header = [&]() {
+#pragma unroll
+        for (int h = 0; h < S; ++h) release_item((int)(cseq % NB));
+    };
 
-    // phase 1 of the tile announced by the next header item, into buffer `buf`; returns the tile (or -1: end of stream)
+    // phase 1 of the tile announced by the next header, into buffer `buf`; returns the tile (or -1: end of stream)
     auto rank_tile = [&](int buf) -> int64_t {
+        DFD_CLK_START(clk_wait);
         const int slot = wait_item();
         const int64_t tile = TIX[slot];
+        // this warp's rows [w * 32K, (w + 1) * 32K) lie in header item w * S / W; all S are held until phase 1 is done
+        const int kslot = wait_item((uint32_t)(w * S / W));
+#pragma unroll
+        for (int h = 1; h < S; ++h) wait_item((uint32_t)h);
+        DFD_CLK_ADD(clk_on, CLK_WAIT_HEADER, clk_wait);
         if (tile < 0) {
-            release_item(slot);
+            release_header();
             return -1;
         }
+        DFD_CLK_START(clk_p1);
         const int64_t row0 = tile * T;
         const int tile_rows = (int)((P.n_rows - row0) < T ? (P.n_rows - row0) : T);
         uint32_t* const TS = (uint32_t*)(smem + L.off_ts) + (uint32_t)buf * (N + 1u);
@@ -865,7 +953,8 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
         for (uint32_t p = lane; p < N; p += 32) wc[p] = 0;
         __syncwarp();
         const int nbits = 32 - __clz(N);
-        const uint64_t* keys = (const uint64_t*)(smem + (uint32_t)slot * slot_bytes);
+        const uint64_t* keys = (const uint64_t*)(smem + (uint32_t)kslot * slot_bytes);
+        const int koff = (w * S / W) * HROWS;  // first tile row of that header item
         uint32_t pos[K];  // (dest << 16 | rank within (warp, dest))
 #pragma unroll
         for (int j = 0; j < K; ++j) {
@@ -873,7 +962,7 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
             const bool valid = t < tile_rows;
             uint32_t d = N;
             if (valid) {
-                const uint64_t h = FAST_I64 ? hash_one_u64(P.st, keys[t]) : row_hash<false>(P.keys, row0 + t, P.st);
+                const uint64_t h = FAST_I64 ? hash_one_u64(P.st, keys[t - koff]) : row_hash<false>(P.keys, row0 + t, P.st);
                 d = mod_n(h, P.mod);
             }
             const unsigned peers = peers_of(d, nbits);
@@ -884,7 +973,7 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
             __syncwarp();
             pos[j] = (d << 16) | (base + rank);
         }
-        release_item(slot);  // key tile consumed
+        release_header();  // key tile consumed
         block_sync<THREADS, BAR>();
         // tile counts = sum of the warps' counts; publish them, then turn warp_cnt into staging bases
         uint32_t carry = 0;
@@ -922,6 +1011,7 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
                 DEST8[sp] = (uint8_t)d;  // N <= 256 in single-pass mode
             }
         }
+        DFD_CLK_ADD(clk_on, CLK_PHASE1, clk_p1);
         return tile;
     };
 
@@ -946,6 +1036,8 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
         const uint32_t* const TS = (const uint32_t*)(smem + L.off_ts) + (uint32_t)buf * (N + 1u);
         const int64_t row0 = tile * T;
         const int tile_rows = (int)((P.n_rows - row0) < T ? (P.n_rows - row0) : T);
+        DFD_CLK_COUNT(clk_on, CLK_TILES);
+        DFD_CLK_START(clk_lb);
         if (threadIdx.x == 0) S_MISC[0] = 0;
         block_sync<THREADS, BAR>();  // (also: SRC16 / DEST8 of this tile are visible, DELTA is free)
         // ---- decoupled look-back: exclusive prefix of every destination over the lower tiles
@@ -1004,6 +1096,8 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
             }
         }
         block_sync<THREADS, BAR>();
+        DFD_CLK_ADD(clk_on, CLK_LOOKBACK, clk_lb);
+        DFD_CLK_START(clk_sc);
         const bool overflow = S_MISC[0] != 0;
         if (overflow && threadIdx.x == 0) *P.overflow_out = 1;  // a region is too small: this tile writes nothing
         const uint16_t* const SRC16 = (const uint16_t*)(smem + L.off_src) + (uint32_t)buf * T;
@@ -1022,9 +1116,11 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
             for (int c = 0; c < P.n_cols; ++c) {
                 void* out_raw = P.cols[c].out;
                 const int cw = P.cols[c].width;
-                const int parts = cw > (int)sizeof(V) ? cw / (int)sizeof(V) : 1;  // (see the producer: wide columns come in row ranges)
+                const int parts = (cw > (int)sizeof(V) ? cw / (int)sizeof(V) : 1) * S;  // (see the producer: columns come in row ranges)
                 for (int h = 0; h < parts; ++h) {
+                    DFD_CLK_START(clk_w);
                     const int slot = wait_item();
+                    DFD_CLK_ADD(clk_on, (FAST_I64 && P.cols[c].in == P.keys.col[0].values) ? CLK_WAIT_KEYCOL : CLK_WAIT_COL, clk_w);
                     const unsigned char* in_raw = smem + (uint32_t)slot * slot_bytes;
                     // one launch moves columns of every width (the rows were ranked once): the element type is per column
                     auto copy_col = [&](auto tag, auto split) {
@@ -1044,17 +1140,7 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
                                 if (orow[k] != SLOT_NONE) st_stream(out + orow[k], in[src[k]]);
                         }
                     };
-                    if (parts > 1) {
-                        if constexpr (sizeof(V) == 8) copy_col(uint4{}, std::true_type{});  // (the host only sends 16-byte columns this way)
-                    } else {
-                        switch (cw) {
-                            case 16: if constexpr (sizeof(V) >= 16) copy_col(uint4{}, std::false_type{}); break;
-                            case 8: if constexpr (sizeof(V) >= 8) copy_col((unsigned long long)0, std::false_type{}); break;
-                            case 4: if constexpr (sizeof(V) >= 4) copy_col((unsigned)0, std::false_type{}); break;
-                            case 2: if constexpr (sizeof(V) >= 2) copy_col((unsigned short)0, std::false_type{}); break;
-                            default: copy_col((unsigned char)0, std::false_type{}); break;
-                        }
-                    }
+                    onepass_by_width<V, S>(cw, parts, copy_col);
                     release_item(slot);
                 }
             }
@@ -1065,9 +1151,11 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
             for (int c = 0; c < P.n_cols; ++c) {
                 const size_t col_out = (size_t)P.cols[c].out;  // local: pointer; peer: byte offset into every window
                 const int cw = P.cols[c].width;
-                const int parts = cw > (int)sizeof(V) ? cw / (int)sizeof(V) : 1;
+                const int parts = (cw > (int)sizeof(V) ? cw / (int)sizeof(V) : 1) * S;  // (see the producer: columns come in row ranges)
                 for (int h = 0; h < parts; ++h) {
+                    DFD_CLK_START(clk_w);
                     const int slot = wait_item();
+                    DFD_CLK_ADD(clk_on, (FAST_I64 && P.cols[c].in == P.keys.col[0].values) ? CLK_WAIT_KEYCOL : CLK_WAIT_COL, clk_w);
                     const unsigned char* in_raw = smem + (uint32_t)slot * slot_bytes;
                     auto copy_col = [&](auto tag, auto split) {
                         using E = decltype(tag);
@@ -1087,24 +1175,16 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
                             }
                         }
                     };
-                    if (parts > 1) {
-                        if constexpr (sizeof(V) == 8) copy_col(uint4{}, std::true_type{});
-                    } else {
-                        switch (cw) {
-                            case 16: if constexpr (sizeof(V) >= 16) copy_col(uint4{}, std::false_type{}); break;
-                            case 8: if constexpr (sizeof(V) >= 8) copy_col((unsigned long long)0, std::false_type{}); break;
-                            case 4: if constexpr (sizeof(V) >= 4) copy_col((unsigned)0, std::false_type{}); break;
-                            case 2: if constexpr (sizeof(V) >= 2) copy_col((unsigned short)0, std::false_type{}); break;
-                            default: copy_col((unsigned char)0, std::false_type{}); break;
-                        }
-                    }
+                    onepass_by_width<V, S>(cw, parts, copy_col);
                     release_item(slot);
                 }
             }
         }
+        DFD_CLK_ADD(clk_on, CLK_SCATTER, clk_sc);
         tile = next;
         buf ^= 1;
     }
+    DFD_CLK_ADD(clk_on, CLK_CONSUMER_TOTAL, clk_total);
     // every CTA draws exactly one ticket >= n_tiles; the last CTA out re-arms the counters for the next launch
     if (threadIdx.x == 0 && atomicAdd(P.lb_ticket + 1, 1u) == gridDim.x - 1) {
         P.lb_ticket[0] = 0;
@@ -1318,9 +1398,9 @@ inline size_t scatter_smem_bytes(uint32_t N, int stage_width, bool peer, bool al
     return off;
 }
 
-template <int THREADS, int K, int NB>
+template <int THREADS, int K, int NB, int S>
 inline size_t onepass_smem_bytes(uint32_t N, int width, bool peer, bool aligned) {
-    return onepass_smem_layout<THREADS, K, NB>(N, (uint32_t)width, peer, aligned).total;
+    return onepass_smem_layout<THREADS, K, NB, S>(N, (uint32_t)width, peer, aligned).total;
 }
 
 }  // namespace dfd

@@ -22,12 +22,17 @@ namespace dfd {
 #ifndef DFD_TILE_MIN_CTAS
 #define DFD_TILE_MIN_CTAS 6
 #endif
-// single-pass kernel: ring depth (tiles in flight per CTA) and resident CTAs per SM
+// single-pass kernel: ring depth (sub-tile items in flight per CTA), items per column of a tile, resident CTAs per SM
 #ifndef DFD_ONEPASS_NB
-#define DFD_ONEPASS_NB 2
+#define DFD_ONEPASS_NB 3
+#endif
+#ifndef DFD_ONEPASS_SPLIT
+#define DFD_ONEPASS_SPLIT 1
 #endif
 #ifndef DFD_ONEPASS_MIN_CTAS
-#define DFD_ONEPASS_MIN_CTAS 4
+// (a register cap of 72 per thread; with NB = 3 a CTA needs 75.5 KB of shared memory at cfg-2, so 2 of them are resident per SM:
+//  the launch sizes the grid by the occupancy API — see DESIGN.md 4.1 for the sweep)
+#define DFD_ONEPASS_MIN_CTAS 3
 #endif
 #ifndef DFD_ONEPASS_K
 #define DFD_ONEPASS_K 10  // rows per consumer thread per tile (tile = 256 x K rows): larger tiles amortise ranking / look-back
@@ -35,6 +40,7 @@ namespace dfd {
 constexpr int ONEPASS_K = DFD_ONEPASS_K;
 constexpr int FOLLOW_MIN_CTAS = 4;  // follow-up k_scatter launches on the single-pass tiling
 constexpr int ONEPASS_NB = DFD_ONEPASS_NB;
+constexpr int ONEPASS_SPLIT = DFD_ONEPASS_SPLIT;
 constexpr int ONEPASS_MIN_CTAS = DFD_ONEPASS_MIN_CTAS;
 constexpr int TILE_THREADS = DFD_TILE_THREADS;
 constexpr int TILE_K = DFD_TILE_K;
@@ -58,8 +64,8 @@ static int launch_scatter_kv(const ScatterParams& sp, int sm_count, size_t smem,
             return set_error(DFD_ERR_INTERNAL, "bit-packed columns take the two-pass k_scatter");
         } else {
             constexpr int KV = ALIGNED ? ONEPASS_KV : ONEPASS_K;
-            auto kern = k_scatter_onepass<TILE_THREADS, ONEPASS_K, KV, ONEPASS_NB, ONEPASS_MIN_CTAS, FAST, V, PEER>;
-            smem = onepass_smem_bytes<TILE_THREADS, ONEPASS_K, ONEPASS_NB>(sp.N, (int)sizeof(V), PEER, ALIGNED);
+            auto kern = k_scatter_onepass<TILE_THREADS, ONEPASS_K, KV, ONEPASS_NB, ONEPASS_SPLIT, ONEPASS_MIN_CTAS, FAST, V, PEER>;
+            smem = onepass_smem_bytes<TILE_THREADS, ONEPASS_K, ONEPASS_NB, ONEPASS_SPLIT>(sp.N, (int)sizeof(V), PEER, ALIGNED);
             if (smem > 227 * 1024) return set_error(DFD_ERR_UNSUPPORTED, "single-pass kernel needs %zu B of shared memory per CTA", smem);
             // (static per instantiation: the attribute and the occupancy are properties of the kernel + smem size)
             static thread_local size_t cfg_smem = 0;
