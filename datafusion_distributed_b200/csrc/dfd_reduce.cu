@@ -210,6 +210,9 @@ extern "C" int dfd_partial_reduce_device(dfd_ctx* c, const dfd_column* in_cols, 
         return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_partial_reduce_device: NULL argument");
     if (n_cols < 1 || n_cols > MAX_REDUCE_COLS || n_keys < 1 || n_keys > MAX_KEYS || n_rows < 0 || n_rows >= 0xffffffffLL || num_partitions < 1)
         return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_partial_reduce_device: bad sizes (columns <= %d, keys <= %d, rows < 2^32)", MAX_REDUCE_COLS, MAX_KEYS);
+    // the table has the next power of two >= 2 * n_rows slots, addressed through a u32 mask: at most 2^32 slots
+    if (n_rows > ((int64_t)1 << 31))
+        return set_error(DFD_ERR_UNSUPPORTED, "dfd_partial_reduce_device: n_rows %lld > 2^31 per call (32-bit hash table slots)", (long long)n_rows);
     ReduceParams P{};
     P.n_cols = n_cols;
     P.n_keys = n_keys;

@@ -187,7 +187,8 @@ int dfd_partition_ids_device(dfd_partitioner* p, const dfd_column* cols, int n_c
  * carries `offsets` (n_rows + 1 entries of the input's offset width) and
  * `values` with `values_bytes` >= the input's byte count; the output is one
  * offsets buffer + one byte buffer in destination order, so destination p is
- * again the zero-copy slice [part_starts[p], part_starts[p+1]). */
+ * again the zero-copy slice [part_starts[p], part_starts[p+1]).
+ * At most 2^32 - 1 rows per call; more: DFD_ERR_UNSUPPORTED, before any allocation or launch. */
 int dfd_partition_device(dfd_partitioner* p, const dfd_column* in_cols, int n_cols,
                          int64_t n_rows, const dfd_column* out_cols, int64_t* part_starts_host);
 const int64_t* dfd_partitioner_part_starts_device(const dfd_partitioner* p);
@@ -199,7 +200,8 @@ const int64_t* dfd_partitioner_part_starts_device(const dfd_partitioner* p);
  * Destination p therefore owns a fixed REGION of every output column: rows
  * [part_starts[p], part_starts[p] + part_counts[p]) with part_starts[p] = p * region_rows — still
  * N contiguous, zero-copy sliceable per-destination buffers, in input order.
- *   out_cols[c] must hold N * region_rows rows, and N * region_rows >= n_rows.
+ *   out_cols[c] must hold N * region_rows rows, and N * region_rows >= n_rows.  Output rows are 32-bit:
+ *   N * region_rows >= 2^32 - 1 is DFD_ERR_UNSUPPORTED (the largest accepted product is 2^32 - 2).
  *   If a destination outgrows its region (skewed keys) nothing is lost: collection re-runs
  *   the kernel with exact regions (part_starts = prefix sums of the now-known counts, dense).
  *   Variable-width payload columns, boolean-only schemas and N > 256 take the two-pass
@@ -432,6 +434,8 @@ int dfd_exchange_phase_ms(dfd_exchange* x, double* out3, uint64_t* n_shuffles);
  * inside a partition is unspecified, like a hash aggregate's).  Feed it to dfd_exchange_gather(DFD_ROUTE_SHUFFLE) — the
  * rows never leave the GPU between Partial aggregation, repartition, PartialReduce and the exchange.
  * Fixed-width non-null keys and states (nullable group keys / states: DFD_ERR_UNSUPPORTED).  Synchronous.
+ * At most 2^31 rows per call (the group table has up to 2^32 slots of 32-bit indices); more: DFD_ERR_UNSUPPORTED,
+ * returned before anything is allocated or launched.
  * Integer SUMs wrap (two's complement, mod 2^64 / 2^128).  Float SUM is the IEEE sum in an unspecified order.  Float
  * MIN / MAX order values by IEEE 754 totalOrder (Rust's f64::total_cmp): -NaN < -inf < ... < -0.0 < +0.0 < ... < +inf
  * < +NaN, NaNs ordered by payload.  So a +NaN wins MAX and a -NaN wins MIN, -0.0 is below +0.0, an all-NaN group yields

@@ -1,11 +1,12 @@
 """CPU checks of the test helpers that other tests build their inputs from: the tile geometry the edge sizes derive from,
-and the crafted PartialReduce group keys that all hash to one slot."""
+the destination tables and row limits of the 32-bit limit tests, and the crafted PartialReduce group keys that all hash
+to one slot."""
 import random
 
 import numpy as np
 
-from tests.util import (M64, REDUCE_HASH_SEED, edge_sizes, keys_on_slot, mix64, reduce_slot_of_i64_key, reduce_table_slots,
-                        tile_geometry, unmix64)
+from tests.util import (M64, PARTITION_MAX_ROWS, REDUCE_HASH_SEED, REDUCE_MAX_ROWS, dest_lut, domain_values, edge_sizes, keys_on_slot,
+                        mix64, onepass_regions_accepted, reduce_slot_of_i64_key, reduce_table_slots, tile_geometry, unmix64)
 
 
 def test_tile_geometry_defaults_and_overrides():
@@ -32,6 +33,42 @@ def test_mix64_matches_the_murmur_finaliser_and_inverts():
     assert [mix64(x) for x in xs] == v.tolist()
     for x in xs:
         assert unmix64(mix64(x)) == x and mix64(unmix64(x)) == x
+
+
+def test_limit_luts_match_the_python_oracle_for_every_domain_value():
+    """The destination tables of the limit tests (C oracle) against the pure-Python ahash restatement, for every key of
+    each domain at each partition count the tests use; a null key goes to destination 0."""
+    from oracle import oracle_py
+
+    for kind, width, Ns in (("u8", 1, (2, 7)), ("i16", 2, (3, 4, 5)), ("i64", 8, (8,))):
+        vals = domain_values(kind)
+        assert len(set(vals.tolist())) == len(vals) == (256 if kind == "u8" else 1 << 16)
+        hashes = [oracle_py.hash_one_int(int(v), width) for v in vals]
+        for N in Ns:
+            lut = dest_lut(kind, N)
+            assert lut.tolist() == [h % N for h in hashes], (kind, N)
+            assert set(lut.tolist()) == set(range(N)), (kind, N)  # every destination is reachable
+    assert oracle_py.create_hashes([("int", 1, [None])], 1) == [0]
+    assert domain_values("i16")[0x8000] == -(1 << 15) and domain_values("i16")[0xFFFF] == -1  # index = the value's bits
+
+
+def test_row_limits_of_the_abi():
+    """The row-count checks the limit tests cross, restated: dense calls take up to 2^32 - 1 rows; single-pass regions
+    need N * region_rows < 2^32 - 1, so 3 x 1 431 655 764 = 2^32 - 4 and 2 x (2^31 - 1) = 2^32 - 2 (the largest accepted
+    product) pass and any product of 2^32 - 1 or more is refused; PartialReduce takes up to 2^31 rows, whose group table
+    of 2^32 slots is the most a u32 mask addresses."""
+    assert PARTITION_MAX_ROWS == 0xFFFFFFFF
+    assert 3 * 1_431_655_764 == (1 << 32) - 4 and onepass_regions_accepted(1_431_655_764, 3, 3_900_000_000)
+    assert 2 * ((1 << 31) - 1) == (1 << 32) - 2 and onepass_regions_accepted((1 << 31) - 1, 2, (1 << 32) - 3)
+    assert not onepass_regions_accepted(1_431_655_765, 3, 64) and 3 * 1_431_655_765 == (1 << 32) - 1
+    assert not onepass_regions_accepted((1 << 32) - 1, 1, 64) and not onepass_regions_accepted(1 << 31, 2, 64)
+    assert not onepass_regions_accepted(1_431_655_764, 3, (1 << 32) - 3)  # too small for the rows
+    # the largest accepted product, over every partition count a single-pass call takes
+    for N in range(1, 257):
+        best = ((1 << 32) - 2) // N
+        assert onepass_regions_accepted(best, N, 1) and not onepass_regions_accepted(best + 1, N, 1)
+    assert reduce_table_slots(REDUCE_MAX_ROWS) == 1 << 32 and reduce_table_slots(REDUCE_MAX_ROWS + 1) == 1 << 33
+    assert reduce_table_slots(REDUCE_MAX_ROWS) - 1 == 0xFFFFFFFF  # the table mask still fits 32 bits
 
 
 def test_crafted_reduce_keys_all_land_on_the_last_slot():

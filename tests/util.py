@@ -73,6 +73,43 @@ def multi_tile_rows():
     return 4 * 7 * sm_count * tile_geometry()[1] + 777  # (ragged last tile)
 
 
+# ------------------------------------------------ 32-bit limits of the ABI ----
+# Restatements of the row-count checks in dfd_api.cu / dfd_reduce.cu, so the limit tests name the boundary they cross.
+
+PARTITION_MAX_ROWS = (1 << 32) - 1  # dfd_partition_device / PartitionJob::prepare: n_rows <= 2^32 - 1
+REDUCE_MAX_ROWS = 1 << 31           # dfd_partial_reduce_device: the group table's slots must fit a u32 mask
+
+
+def onepass_regions_accepted(region_rows: int, N: int, n_rows: int) -> bool:
+    """dfd_partition_device_onepass's region check: every row fits, and N * region_rows < 2^32 - 1 (32-bit output rows,
+    0xffffffff is the kernel's empty-slot sentinel)."""
+    return region_rows >= 1 and region_rows * N >= n_rows and region_rows * N < (1 << 32) - 1
+
+
+# Small key domains for the limit tests: the destination of every possible key is computed once by the C oracle, and the
+# GPU then derives a row's destination as LUT[key] — exact at any row count, and independent of the kernels under test.
+
+def domain_values(kind: str) -> np.ndarray:
+    """Every key of a domain, at its LUT index: "u8" = all 256 uint8 values, "i16" = all 65 536 int16 values (index =
+    the value's bits as uint16), "i64" = 65 536 seeded int64 values (index = an int16 row's bits as uint16)."""
+    if kind == "u8":
+        return np.arange(256, dtype=np.uint8)
+    if kind == "i16":
+        return np.arange(1 << 16, dtype=np.uint16).view(np.int16)
+    if kind == "i64":
+        return np.random.Generator(np.random.PCG64(2024)).integers(-(1 << 63), (1 << 63) - 1, 1 << 16, dtype=np.int64, endpoint=True)
+    raise ValueError(kind)
+
+
+def dest_lut(kind: str, N: int) -> np.ndarray:
+    """Destination (create_hashes % N, the C oracle) of every key of domain `kind`, as int32 indexed like domain_values.
+    A null key hashes to 0 and goes to destination 0."""
+    from oracle import oracle as orc
+
+    v = domain_values(kind)
+    return orc.partition_ids([v], len(v), N).astype(np.int32)
+
+
 # ---------------------------------------------- PartialReduce group hashing ----
 # Restatement of dfd_reduce.cu's key_hash for one 8-byte key, and its inverse, to craft keys that land on a chosen slot.
 
