@@ -60,8 +60,14 @@ template <bool FAST, typename V, bool PEER, bool ALIGNED, int MODE>
 static int launch_scatter_kv(const ScatterParams& sp, int sm_count, size_t smem, cudaStream_t stream) {
     cudaError_t e;
     if constexpr (MODE == 1) {
+        // run_onepass launches a ring of min(widest column, 8) bytes and takes the fast key path only with an 8-byte ring:
+        // the other single-pass instantiations are never launched, so they are not compiled
         if constexpr (std::is_same<V, BitColumn>::value) {
             return set_error(DFD_ERR_INTERNAL, "bit-packed columns take the two-pass k_scatter");
+        } else if constexpr (sizeof(V) > 8) {
+            return set_error(DFD_ERR_INTERNAL, "the single-pass ring is at most 8 bytes wide");
+        } else if constexpr (FAST && sizeof(V) < 8) {
+            return set_error(DFD_ERR_INTERNAL, "the single-pass fast key path needs an 8-byte ring");
         } else {
             constexpr int KV = ALIGNED ? ONEPASS_KV : ONEPASS_K;
             auto kern = k_scatter_onepass<TILE_THREADS, ONEPASS_K, KV, ONEPASS_NB, ONEPASS_SPLIT, ONEPASS_MIN_CTAS, FAST, V, PEER>;

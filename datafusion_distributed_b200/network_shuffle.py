@@ -198,7 +198,8 @@ class NetworkShuffleExec:
         """`dfd_shuffle_device_onepass`: the NCCL-free fused shuffle.  Fixed-width non-null columns take the single-pass
         kernel (asynchronous); nullable / boolean / string columns take the push transport.  `nullable[i]` is the
         SCHEMA's nullable flag of column i (every worker must pass the same; default: this worker's columns that
-        carry a validity bitmap).  Complete it with `collect()`."""
+        carry a validity bitmap).  Complete it with `collect()`; `in_cols` must stay allocated until then, because a
+        shuffle whose sub-window overflowed re-runs from them inside `collect()`."""
         if len(self.input_stage.tasks) != exchange.world or self.task_count != exchange.world:
             raise ValueError("this exchange runs one producer and one consumer task per GPU worker")
         P = self.properties.partition_count

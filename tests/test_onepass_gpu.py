@@ -18,10 +18,15 @@ def dev_cols(ctx, arrays):
     return [dfd.DeviceColumn.from_arrow(ctx, a if isinstance(a, pa.Array) else pa.array(a)) for a in arrays]
 
 
-def check_against_oracle(ctx, arrays, key_cols, N, region_rows=None):
+def check_against_oracle(ctx, arrays, key_cols, N, region_rows=None, two_pass=False):
+    """Single-pass partition (or, with two_pass, the dense partition()) of `arrays` against the oracle."""
     n = len(arrays[0])
     part = dfd.HashPartitioner(ctx, dfd.Partitioning.Hash(key_cols, N))
-    outs, starts, counts = part.partition_onepass(dev_cols(ctx, arrays), n, region_rows)
+    if two_pass:
+        outs, part_starts = part.partition(dev_cols(ctx, arrays), n)
+        starts, counts = part_starts[:-1], np.diff(part_starts)
+    else:
+        outs, starts, counts = part.partition_onepass(dev_cols(ctx, arrays), n, region_rows)
     keys = [arrays[k] for k in key_cols]
     dest = orc.partition_ids(keys, n, N)
     order, ref_starts = expected_partitions(dest, N)

@@ -5,8 +5,9 @@ import random
 
 import numpy as np
 
-from tests.util import (M64, PARTITION_MAX_ROWS, REDUCE_HASH_SEED, REDUCE_MAX_ROWS, dest_lut, domain_values, edge_sizes, keys_on_slot,
-                        mix64, onepass_regions_accepted, reduce_slot_of_i64_key, reduce_table_slots, tile_geometry, unmix64)
+from tests.util import (M64, PARTITION_MAX_ROWS, REDUCE_HASH_SEED, REDUCE_MAX_ROWS, ScatterInst, dest_lut, domain_values, edge_sizes,
+                        keys_on_slot, mix64, onepass_regions_accepted, parse_scatter_name, reduce_slot_of_i64_key, reduce_table_slots,
+                        scatter_inst, scatter_instances, tile_geometry, unmix64, use_aligned)
 
 
 def test_tile_geometry_defaults_and_overrides():
@@ -17,6 +18,27 @@ def test_tile_geometry_defaults_and_overrides():
     sizes = set(edge_sizes({}))
     assert {1535, 1536, 1537, 3072, 3073, 2559, 2560, 2561, 5120, 5121} <= sizes and {0, 1, 31, 32, 33, 2047, 2048, 2049} <= sizes
     assert {511, 512, 513, 1024, 1025} <= set(edge_sizes({"DFD_NVCC_DEFS": "-DDFD_TILE_THREADS=128 -DDFD_TILE_K=4"}))
+
+
+def test_scatter_kernel_names_parse_in_every_demangler_format():
+    """cu++filt (the library's symbol table) and the GNU demangler (profiler kernel names) spell template arguments
+    differently; both, and the mangled name, give the same instantiation."""
+    want = ScatterInst("k_scatter_onepass", 10, 14, True, "u32", True)
+    assert parse_scatter_name("void dfd::k_scatter_onepass<(int)256, (int)10, (int)14, (int)3, (int)1, (int)3, (bool)1, unsigned int, "
+                              "(bool)1>(dfd::ScatterParams)") == want
+    assert parse_scatter_name("void dfd::k_scatter_onepass<256, 10, 14, 3, 1, 3, true, unsigned int, true>(dfd::ScatterParams)") == want
+    assert scatter_instances(["_ZN3dfd17k_scatter_onepassILi256ELi10ELi14ELi3ELi1ELi3ELb1EjLb1EEEvNS_13ScatterParamsE", "k_scan_tiles"]) == {want}
+    assert parse_scatter_name("void dfd::k_scatter<256, 6, 10, 6, false, dfd::BitColumn, false>(dfd::ScatterParams)") == \
+        ScatterInst("k_scatter", 6, 10, False, "bit", False)
+    assert parse_scatter_name("void dfd::k_scatter<(int)256, (int)10, (int)10, (int)4, (bool)0, uint4, (bool)1>(dfd::ScatterParams)") == \
+        ScatterInst("k_scatter", 10, 10, False, "uint4", True)
+    assert parse_scatter_name("void dfd::k_tile_hist<256, 6, true, 2>(dfd::KeySet, unsigned int)") is None
+    # the dispatch restatement names instantiations the same way
+    assert scatter_inst(1, True, "u32", True, True, {}) == want
+    assert scatter_inst(0, False, "bit", False, True, {}) == ScatterInst("k_scatter", 6, 10, False, "bit", False)
+    assert scatter_inst(2, False, "u8", True, True, {}) == ScatterInst("k_scatter", 10, 14, False, "u8", True)
+    assert use_aligned(16, True, {}) and not use_aligned(17, True, {}) and not use_aligned(8, False, {})
+    assert use_aligned(8, False, {"DFD_ALIGNED_WRITEOUT": "1"}) and not use_aligned(8, True, {"DFD_ALIGNED_WRITEOUT": "0"})
 
 
 def test_mix64_matches_the_murmur_finaliser_and_inverts():

@@ -4,6 +4,8 @@ from __future__ import annotations
 import json
 import os
 import re
+import subprocess
+from typing import NamedTuple
 
 import numpy as np
 
@@ -35,12 +37,8 @@ def expected_partitions(dest: np.ndarray, num_partitions: int):
 
 # ------------------------------------------------------------ tile geometry ----
 
-def tile_geometry(env=None):
-    """(two-pass tile rows, single-pass tile rows) of the library as build.py compiles it: the defaults of
-    csrc/dfd_launch.cuh, overridden by the -DNAME=VALUE options of DFD_NVCC_DEFS (and, for the single-pass K, of
-    DFD_NVCC_DEFS_ONEPASS), which build.py passes to nvcc.  The tile-sweep scripts rebuild with other geometries; the
-    edge sizes of the scatter tests follow them through this."""
-    env = os.environ if env is None else env
+def _launch_defines(env):
+    """The tile-geometry macros of csrc/dfd_launch.cuh as build.py compiles them (see tile_geometry)."""
     with open(LAUNCH_HEADER) as f:
         src = f.read()
     vals = {m.group(1): int(m.group(2)) for m in re.finditer(r"#define\s+(DFD_\w+)\s+(\d+)", src)}
@@ -48,6 +46,16 @@ def tile_geometry(env=None):
         for m in re.finditer(r"-D(DFD_\w+)=(\d+)", env.get(var, "")):
             if var == "DFD_NVCC_DEFS" or m.group(1) == "DFD_ONEPASS_K":
                 vals[m.group(1)] = int(m.group(2))
+    vals["ALIGNED_MAX_N"] = int(re.search(r"ALIGNED_MAX_N\s*=\s*(\d+)", src).group(1))
+    return vals
+
+
+def tile_geometry(env=None):
+    """(two-pass tile rows, single-pass tile rows) of the library as build.py compiles it: the defaults of
+    csrc/dfd_launch.cuh, overridden by the -DNAME=VALUE options of DFD_NVCC_DEFS (and, for the single-pass K, of
+    DFD_NVCC_DEFS_ONEPASS), which build.py passes to nvcc.  The tile-sweep scripts rebuild with other geometries; the
+    edge sizes of the scatter tests follow them through this."""
+    vals = _launch_defines(os.environ if env is None else env)
     threads = vals["DFD_TILE_THREADS"]
     return threads * vals["DFD_TILE_K"], threads * vals["DFD_ONEPASS_K"]
 
@@ -71,6 +79,137 @@ def multi_tile_rows():
 
     sm_count = torch.cuda.get_device_properties(0).multi_processor_count
     return 4 * 7 * sm_count * tile_geometry()[1] + 777  # (ragged last tile)
+
+
+# ------------------------------------------------------ scatter instantiations ----
+# The scatter kernels are templates, and launch_scatter_kv (csrc/dfd_launch.cuh) picks one instantiation per launch from
+# MODE (two-pass, single-pass, follow-up), FAST (Int64 key path), V (element type), PEER and ALIGNED.  An instantiation is
+# named by the template arguments that tell them apart: K (rows per thread of the tiling: two-pass or single-pass), KV
+# (KV > K: the aligned write-out), FAST, V and PEER.  The same parser reads the library's symbol table and the kernel
+# names a profiler records, so a test can check which instantiations exist and which ones an input ran.
+
+class ScatterInst(NamedTuple):
+    kernel: str  # "k_scatter" (two-pass and follow-up launches) or "k_scatter_onepass"
+    K: int
+    KV: int
+    fast: bool
+    V: str  # one of WIDTH_V's values
+    peer: bool
+
+    @property
+    def aligned(self) -> bool:
+        return self.KV > self.K
+
+
+WIDTH_V = {8: "u64", 4: "u32", 16: "uint4", 2: "u16", 1: "u8", 0: "bit"}  # launch_scatter_w: column width -> V (0: bit column)
+_CXX_V = {"unsigned char": "u8", "unsigned short": "u16", "unsigned int": "u32", "unsigned long": "u64", "unsigned long long": "u64",
+          "uint4": "uint4", "dfd::BitColumn": "bit"}
+_SCATTER_NAME = re.compile(r"\bdfd::(k_scatter(?:_onepass)?)<(.*)>\s*\((?:const\s+)?dfd::ScatterParams\)")
+
+
+def _cuda_tool(name: str) -> str:
+    """A CUDA toolkit binary next to the nvcc that build.py uses."""
+    path = os.path.join(os.path.dirname(os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")), name)
+    return path if os.path.exists(path) else name
+
+
+def _int_arg(a: str) -> int:
+    a = re.sub(r"^\((?:int|bool|unsigned int)\)", "", a.strip())  # cu++filt writes (int)256 / (bool)1, the GNU demangler 256 / true
+    return {"true": 1, "false": 0}[a] if a in ("true", "false") else int(a.rstrip("u"))
+
+
+def parse_scatter_name(name: str):
+    """ScatterInst of a demangled scatter kernel name such as `void dfd::k_scatter_onepass<(int)256, (int)10, (int)14,
+    (int)3, (int)1, (int)3, (bool)1, unsigned int, (bool)1>(dfd::ScatterParams)`; None for any other kernel.
+    k_scatter<THREADS, K, KV, MIN_CTAS, FAST, V, PEER>, k_scatter_onepass<THREADS, K, KV, NB, SPLIT, MIN_CTAS, FAST, V, PEER>."""
+    m = _SCATTER_NAME.search(name)
+    if not m:
+        return None
+    a = [s.strip() for s in m.group(2).split(",")]
+    return ScatterInst(m.group(1), _int_arg(a[1]), _int_arg(a[2]), bool(_int_arg(a[-3])), _CXX_V[a[-2]], bool(_int_arg(a[-1])))
+
+
+def scatter_instances(names) -> set:
+    """The scatter instantiations among kernel names, demangled or mangled (those are demangled by cu++filt)."""
+    names = list(names)
+    mangled = [n for n in names if n.startswith("_Z")]
+    if mangled:
+        out = subprocess.run([_cuda_tool("cu++filt")], input="\n".join(mangled) + "\n", capture_output=True, text=True, check=True).stdout
+        names = [n for n in names if not n.startswith("_Z")] + out.splitlines()
+    return {i for i in map(parse_scatter_name, names) if i is not None}
+
+
+def compiled_scatter_instances(lib_path: str) -> set:
+    """Every scatter instantiation in the library's device code (cuobjdump -symbols)."""
+    out = subprocess.run([_cuda_tool("cuobjdump"), "-symbols", lib_path], capture_output=True, text=True, check=True).stdout
+    return scatter_instances(re.findall(r"\b(_Z\S*k_scatter\S*)", out))
+
+
+def scatter_inst(mode: int, fast: bool, V: str, peer: bool, aligned: bool, env=None) -> ScatterInst:
+    """The instantiation launch_scatter_kv<FAST, V, PEER, ALIGNED, MODE> launches (dfd_launch.cuh:59-106): MODE 0 is
+    k_scatter on the two-pass tiling, 1 k_scatter_onepass and 2 k_scatter on the single-pass tiling; the aligned
+    write-out pads KV by ceil(62 * ALIGNED_MAX_N / THREADS) rows per thread (TILE_KV / ONEPASS_KV, dfd_launch.cuh:50-52)."""
+    d = _launch_defines(os.environ if env is None else env)
+    threads = d["DFD_TILE_THREADS"]
+    K = d["DFD_TILE_K"] if mode == 0 else d["DFD_ONEPASS_K"]
+    KV = K + (62 * d["ALIGNED_MAX_N"] + threads - 1) // threads if aligned else K
+    return ScatterInst("k_scatter_onepass" if mode == 1 else "k_scatter", K, KV, bool(fast), V, bool(peer))
+
+
+def use_aligned(N: int, peer: bool, env=None) -> bool:
+    """dfd_api.cu:133-137: the aligned write-out runs up to ALIGNED_MAX_N destinations, for peer launches only unless
+    DFD_ALIGNED_WRITEOUT=0/1 forces it (read once per process by the library)."""
+    env = os.environ if env is None else env
+    if N > _launch_defines(env)["ALIGNED_MAX_N"]:
+        return False
+    forced = env.get("DFD_ALIGNED_WRITEOUT")
+    return int(forced) != 0 if forced is not None else peer
+
+
+_ROUTES = {(0, False): "dfd_partition_device, and the local partition of the NCCL mode and the push transport (dfd_exchange.cu:1118)",
+           (0, True): "EXCHANGE_FUSED (dfd_exchange.cu:682) and the exact re-run after a single-pass sub-window overflow (:1502)",
+           (1, False): "dfd_partition_device_onepass",
+           (1, True): "dfd_shuffle_device_onepass with fixed-width non-null columns (onepass_supported, dfd_exchange.cu:705)",
+           (2, False): "dfd_partition_device_onepass: bit columns, or fixed-width columns past the first MAX_COLS_PER_LAUNCH",
+           (2, True): "dfd_shuffle_device_onepass: fixed-width columns past the first MAX_COLS_PER_LAUNCH"}
+ALIGNED_LOCAL_REASON = "env-only: DFD_ALIGNED_WRITEOUT=1 (use_aligned, dfd_api.cu:133-137) is what turns on the aligned write-out of a local launch"
+
+
+def scatter_dispatch(env=None):
+    """Restatement of the scatter dispatch of dfd_api.cu (run_scatter, run_onepass) and dfd_launch.cuh.  Returns
+    ({instantiation: route} for every instantiation an input reaches, {instantiation: reason} for those reached only
+    under an environment override).  The rules:
+    - widths: run_scatter and the follow-ups launch one group per column width {8, 4, 16, 2, 1, 0 = bit columns}
+      (dfd_api.cu:360, :475), each mapped to V by launch_scatter_w (dfd_launch.cuh:116-128);
+    - bit columns (Boolean values, validity bitmaps) exist only in local calls: peer calls reject them
+      (dfd_api.cu:189, :226), and neither they nor single-pass launches have a bit instantiation (dfd_launch.cuh:123);
+    - the single-pass launch moves the first MAX_COLS_PER_LAUNCH fixed-width columns with ring_w = min(widest, 8)
+      (dfd_api.cu:454, :466): V is u8, u16, u32 or u64, never uint4;
+    - it takes the FAST key path only with an 8-byte ring (`fast_i64 && ring_w >= 8`, dfd_api.cu:467; the guards at
+      dfd_launch.cuh:65-71 compile no single-pass kernel outside these two rules); two-pass and
+      follow-up launches take it whenever the key is fast_i64 (dfd_api.cu:375, :487);
+    - follow-up launches (MODE 2) move the bit columns and the fixed-width columns past the first launch (dfd_api.cu:454);
+    - ALIGNED = use_aligned(N, PEER) (dfd_launch.cuh:110): for peer launches N <= 16 and N > 16 both occur; a local
+      launch is aligned only under DFD_ALIGNED_WRITEOUT=1."""
+    reach, env_only = {}, {}
+    for mode in (0, 1, 2):
+        for width, V in WIDTH_V.items():
+            if mode == 1 and width not in (1, 2, 4, 8):
+                continue
+            for peer in (False, True):
+                if peer and width == 0:
+                    continue
+                for fast in (False, True):
+                    if mode == 1 and fast and width != 8:
+                        continue
+                    for aligned in (False, True):
+                        inst = scatter_inst(mode, fast, V, peer, aligned, env)
+                        if aligned and not peer:
+                            env_only[inst] = ALIGNED_LOCAL_REASON
+                        else:
+                            reach[inst] = f"{_ROUTES[mode, peer]}; V = {V}, {'Int64 fast key' if fast else 'generic key'}" + (
+                                f", N {'<=' if aligned else '>'} 16" if peer else "")
+    return reach, env_only
 
 
 # ------------------------------------------------ 32-bit limits of the ABI ----
