@@ -125,7 +125,7 @@ SIGNATURES = {
     "dfd_partitioner_destroy": (None, [_VP]),
     "dfd_partitioner_num_partitions": (C.c_uint32, [_VP]),
     "dfd_partitioner_set_key_hash_mode": (C.c_int, [_VP, C.c_int, C.c_int]),
-    "dfd_partitioner_set_key_dictionary": (C.c_int, [_VP, C.c_int, _VP, _VP]),
+    "dfd_partitioner_set_key_dictionary": (C.c_int, [_VP, C.c_int, _VP, _VP, C.c_int]),
     "dfd_hash_columns_device": (C.c_int, [_VP, C.POINTER(DfdColumn), C.c_int, C.c_int64, C.POINTER(C.c_uint64), _VP]),
     "dfd_partition_ids_device": (C.c_int, [_VP, C.POINTER(DfdColumn), C.c_int, C.c_int64, _VP]),
     "dfd_partition_device": (C.c_int, [_VP, C.POINTER(DfdColumn), C.c_int, C.c_int64, C.POINTER(DfdColumn), C.POINTER(C.c_int64)]),

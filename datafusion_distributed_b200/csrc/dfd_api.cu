@@ -87,13 +87,14 @@ static int build_keyset(const dfd_partitioner* p, const dfd_column* cols, int n_
         kc.offset = c.offset;
         kc.kind = c.kind;
         kc.width = (int16_t)c.width;
-        kc.mode = (int16_t)p->key_modes[k];
+        kc.mode = (int8_t)p->key_modes[k];
         if (kc.mode == KEY_HASH_DICTIONARY) {
             if (c.kind != DFD_COL_FIXED || (c.width != 1 && c.width != 2 && c.width != 4 && c.width != 8))
                 return set_error(DFD_ERR_INVALID_ARGUMENT, "key column %d: dictionary indices must be a fixed-width integer column", ci);
             if (!p->key_dicts[k].hashes) return set_error(DFD_ERR_INVALID_ARGUMENT, "key column %d: no dictionary set (dfd_partitioner_set_key_dictionary)", ci);
             kc.offsets = p->key_dicts[k].hashes;
             kc.dict_validity = p->key_dicts[k].validity;
+            kc.index_unsigned = p->key_dicts[k].index_unsigned ? 1 : 0;
         }
         switch (c.kind) {
             case DFD_COL_FIXED:
@@ -599,15 +600,23 @@ int dfd::partition_device_locked(Partitioner* p, const dfd_column* in_cols, int 
     return job.run_scatter(p->d_part_starts, nullptr, 1, 1, nullptr);
 }
 
-int dfd::hash_columns_locked(Ctx* c, const dfd_column* cols, int n_cols, int64_t n_rows, const uint64_t* seeds, uint64_t* hashes_device,
+int dfd::hash_columns_locked(Ctx* c, const dfd_column* in_cols, int n_cols, int64_t n_rows, const uint64_t* seeds, uint64_t* hashes_device,
                              cudaStream_t stream) {
-    if (!cols || n_cols < 1 || n_cols > MAX_KEYS || n_rows < 0 || !hashes_device)
+    if (!in_cols || n_cols < 1 || n_cols > MAX_KEYS || n_rows < 0 || !hashes_device)
         return set_error(DFD_ERR_INVALID_ARGUMENT, "hash_columns: bad arguments");
     dfd_partitioner tmp;
     tmp.ctx = c;
     tmp.N = 1;
     for (int i = 0; i < n_cols; ++i) tmp.key_cols.push_back(i);
     tmp.key_modes.assign((size_t)n_cols, DFD_KEY_HASH_PLAIN);
+    dfd_column cols[MAX_KEYS];
+    for (int i = 0; i < n_cols; ++i) {  // interval values: a FIXED column hashed field by field
+        cols[i] = in_cols[i];
+        if (cols[i].kind == COL_INTERVAL_DAY_TIME || cols[i].kind == COL_INTERVAL_MONTH_DAY_NANO) {
+            tmp.key_modes[(size_t)i] = cols[i].kind == COL_INTERVAL_DAY_TIME ? DFD_KEY_HASH_INTERVAL_DAY_TIME : DFD_KEY_HASH_INTERVAL_MONTH_DAY_NANO;
+            cols[i].kind = DFD_COL_FIXED;
+        }
+    }
     tmp.key_dicts.assign((size_t)n_cols, dfd_partitioner::KeyDict{});
     static const uint64_t PI2[4] = {0x452821e638d01377ULL, 0xbe5466cf34e90c6cULL, 0xc0ac29b7c97c50ddULL, 0x3f84d5b5b5470917ULL};
     uint64_t sd[4] = {0, 0, 0, 0};
@@ -874,7 +883,8 @@ void dfd_partitioner_destroy(dfd_partitioner* p) {
 
 uint32_t dfd_partitioner_num_partitions(const dfd_partitioner* p) { return p ? p->N : 0; }
 
-int dfd_partitioner_set_key_dictionary(dfd_partitioner* p, int key_index, const uint64_t* dict_hashes_device, const uint8_t* dict_validity_device) {
+int dfd_partitioner_set_key_dictionary(dfd_partitioner* p, int key_index, const uint64_t* dict_hashes_device, const uint8_t* dict_validity_device,
+                                       int index_is_unsigned) {
     if (!p) return set_error(DFD_ERR_INVALID_ARGUMENT, "partitioner is NULL");
     if (key_index < 0 || key_index >= (int)p->key_cols.size()) return set_error(DFD_ERR_INVALID_ARGUMENT, "key index %d out of range", key_index);
     std::lock_guard<std::mutex> lk(p->ctx->mu);
@@ -884,12 +894,15 @@ int dfd_partitioner_set_key_dictionary(dfd_partitioner* p, int key_index, const 
         return DFD_OK;
     }
     p->key_modes[(size_t)key_index] = KEY_HASH_DICTIONARY;
-    p->key_dicts[(size_t)key_index] = dfd_partitioner::KeyDict{dict_hashes_device, dict_validity_device};
+    p->key_dicts[(size_t)key_index] = dfd_partitioner::KeyDict{dict_hashes_device, dict_validity_device, index_is_unsigned != 0};
     return DFD_OK;
 }
 
 int dfd_hash_columns_device(dfd_ctx* c, const dfd_column* cols, int n_cols, int64_t n_rows, const uint64_t* seeds, uint64_t* hashes_device) {
     if (!c) return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_hash_columns_device: ctx is NULL");
+    for (int i = 0; cols && i < n_cols; ++i)  // (the internal interval kinds are not part of the C ABI)
+        if (cols[i].kind < DFD_COL_FIXED || cols[i].kind > DFD_COL_BINARY)
+            return set_error(DFD_ERR_UNSUPPORTED, "dfd_hash_columns_device: column %d: unknown kind %d", i, cols[i].kind);
     CTX_GUARD(c);
     return hash_columns_locked(c, cols, n_cols, n_rows, seeds, hashes_device, c->stream);
 }

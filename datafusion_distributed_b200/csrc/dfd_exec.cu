@@ -52,6 +52,7 @@ struct FieldInfo {
     int32_t child_width = 0;       // list child: 0 = Utf8 / Binary (offsets + bytes), > 0 = fixed-width primitive of that many bytes
     bool nodev() const { return list; }
     bool dict = false;             // dictionary-encoded: `format` is the index type, dict_* describe the values
+    bool dict_index_unsigned = false;  // UInt8/16/32/64 indices ("C" "S" "I" "L")
     std::string dict_format;
     int64_t dict_flags = 0;
     int32_t dict_kind = DFD_COL_FIXED, dict_width = 0;
@@ -62,6 +63,12 @@ struct FieldInfo {
 // LargeBinary and FixedSizeBinary values are hashed by DataFusion as byte slices with a length prefix; the device hashes a
 // LARGE_UTF8 column as strings and a FIXED column as an integer: such columns travel as payload but cannot be hash keys.
 bool hashable_format(const char* f) { return f[0] != 'Z' && f[0] != 'w'; }
+
+// Interval(DayTime) / Interval(MonthDayNano) values hash field by field (arrow's derived Hash), as keys and as the values of
+// a dictionary key alike; everything else is one integer / byte-slice write.
+int32_t interval_key_mode(const std::string& f) {
+    return f == "tiD" ? DFD_KEY_HASH_INTERVAL_DAY_TIME : f == "tin" ? DFD_KEY_HASH_INTERVAL_MONTH_DAY_NANO : DFD_KEY_HASH_PLAIN;
+}
 
 // Arrow format string -> physical layout (Arrow C data interface, "Data type description")
 bool parse_format(const char* f, int32_t* kind, int32_t* width) {
@@ -701,7 +708,7 @@ int flush_current(dfd_repartition_exec* x) {
     for (size_t i = 0; i < C; ++i)  // dictionary keys of this chunk (caller holds the context lock: set the fields directly)
         if (x->fields[i].dict && x->key_of_field[i] >= 0) {
             x->part->key_modes[(size_t)x->key_of_field[i]] = dfd::KEY_HASH_DICTIONARY;
-            x->part->key_dicts[(size_t)x->key_of_field[i]] = dfd_partitioner::KeyDict{s.dict_hashes[i], s.dict_valid[i]};
+            x->part->key_dicts[(size_t)x->key_of_field[i]] = dfd_partitioner::KeyDict{s.dict_hashes[i], s.dict_valid[i], x->fields[i].dict_index_unsigned};
         }
     int rc = partition_device_locked(x->part, in.data(), (int)D, s.rows, out.data(), c->stream, /*var_bytes_known=*/true);
     if (rc) return fail(x, rc, dfd_last_error());
@@ -1012,7 +1019,10 @@ int stage_rows(dfd_repartition_exec* x, const ArrowArray* b, int64_t start, int6
             if (dvar) XCUDA(x, cudaMemcpyAsync(db + o_off, d->buffers[1], (size_t)(dn + 1) * dow, cudaMemcpyHostToDevice, x->s_h2d), "H2D dictionary offsets");
             if (vbytes) XCUDA(x, cudaMemcpyAsync(db + o_data, d->buffers[dvar ? 2 : 1], vbytes, cudaMemcpyHostToDevice, x->s_h2d), "H2D dictionary values");
             if (dhv) XCUDA(x, cudaMemcpyAsync(db + o_valid, d->buffers[0], (size_t)((dn + 7) / 8), cudaMemcpyHostToDevice, x->s_h2d), "H2D dictionary validity");
-            dfd_column dc{f.dict_kind, f.dict_width, db + o_data, dvar ? (void*)(db + o_off) : nullptr, dhv ? (uint8_t*)(db + o_valid) : nullptr, d->offset,
+            const int32_t dmode = interval_key_mode(f.dict_format);  // interval values hash field by field, as interval keys do
+            const int32_t hkind = dmode == DFD_KEY_HASH_INTERVAL_DAY_TIME ? COL_INTERVAL_DAY_TIME
+                                  : dmode == DFD_KEY_HASH_INTERVAL_MONTH_DAY_NANO ? COL_INTERVAL_MONTH_DAY_NANO : f.dict_kind;
+            dfd_column dc{hkind, f.dict_width, db + o_data, dvar ? (void*)(db + o_off) : nullptr, dhv ? (uint8_t*)(db + o_valid) : nullptr, d->offset,
                           (int64_t)vbytes};
             rc2 = hash_columns_locked(x->ctx, &dc, 1, d->length, nullptr, (uint64_t*)(db + o_hash), x->s_h2d);
             if (rc2) return fail(x, rc2, dfd_last_error());
@@ -1178,6 +1188,7 @@ int dfd_repartition_exec_create(dfd_ctx* ctx, const struct ArrowSchema* schema, 
             if (f.kind != DFD_COL_FIXED || !strchr("cCsSiIlL", f.format[0]) || f.format[1])
                 return set_error(DFD_ERR_UNSUPPORTED, "column %lld (%s): dictionary index type '%s' is not an integer", (long long)i, f.name.c_str(), f.format.c_str());
             f.dict = true;
+            f.dict_index_unsigned = strchr("CSIL", f.format[0]) != nullptr;
             f.dict_format = d->format ? d->format : "";
             f.dict_flags = d->flags;
             if (d->dictionary || d->n_children > 0 || !parse_format(f.dict_format.c_str(), &f.dict_kind, &f.dict_width))
@@ -1224,8 +1235,7 @@ int dfd_repartition_exec_create(dfd_ctx* ctx, const struct ArrowSchema* schema, 
     int rc = dfd_partitioner_create(ctx, num_partitions, dev_keys.data(), n_keys, nullptr, &x->part);
     if (rc) return rc;  // (x has no CUDA resources yet; unique_ptr frees it)
     for (int k = 0; k < n_keys; ++k) {  // interval keys hash field by field (arrow's derived Hash), not as one integer
-        const std::string& fmt = x->fields[(size_t)key_cols[k]].format;
-        const int mode = fmt == "tiD" ? DFD_KEY_HASH_INTERVAL_DAY_TIME : fmt == "tin" ? DFD_KEY_HASH_INTERVAL_MONTH_DAY_NANO : DFD_KEY_HASH_PLAIN;
+        const int mode = interval_key_mode(x->fields[(size_t)key_cols[k]].format);  // (a dictionary field's format is its index type)
         if (mode != DFD_KEY_HASH_PLAIN && (rc = dfd_partitioner_set_key_hash_mode(x->part, k, mode))) {
             dfd_partitioner_destroy(x->part);
             x->part = nullptr;

@@ -32,17 +32,18 @@ struct KeyCol {
     int64_t offset;
     int32_t kind;
     int16_t width;
-    int16_t mode;  // KEY_HASH_*: how a fixed-width value is fed to the hasher
+    int8_t mode;              // KEY_HASH_*: how a fixed-width value is fed to the hasher
+    uint8_t index_unsigned;   // KEY_HASH_DICTIONARY: the indices are UInt8/16/32/64 (zero-extended), else signed
     const uint8_t* dict_validity;  // KEY_HASH_DICTIONARY: validity bitmap of the dictionary VALUES (or nullptr); `offsets` = their u64 hashes
 };
 
 // A fixed-width key is normally ONE write_u{8..128}.  Arrow's interval structs derive `Hash`, i.e. one write
 // per field (arrow-buffer IntervalDayTime {i32, i32}, IntervalMonthDayNano {i32, i32, i64}; DataFusion hash_utils
 // `hash_value!(.., IntervalDayTime, IntervalMonthDayNano)` -> `state.hash_one(self)`).
-// KEY_HASH_DICTIONARY: the column holds dictionary INDICES (signed, `width` bytes); DataFusion's hash_dictionary hashes the
-// dictionary values once (create_hashes over the values array) and a row takes dict_hashes[index]; a null index or a null
-// dictionary value leaves the running hash untouched.
-enum KeyHashMode : int16_t { KEY_HASH_PLAIN = 0, KEY_HASH_INTERVAL_DAY_TIME = 1, KEY_HASH_INTERVAL_MONTH_DAY_NANO = 2, KEY_HASH_DICTIONARY = 3 };
+// KEY_HASH_DICTIONARY: the column holds dictionary INDICES (`width` bytes, signed or unsigned per `index_unsigned`);
+// DataFusion's hash_dictionary hashes the dictionary values once (create_hashes over the values array) and a row takes
+// dict_hashes[key.as_usize()]; a null index or a null dictionary value leaves the running hash untouched.
+enum KeyHashMode : int8_t { KEY_HASH_PLAIN = 0, KEY_HASH_INTERVAL_DAY_TIME = 1, KEY_HASH_INTERVAL_MONTH_DAY_NANO = 2, KEY_HASH_DICTIONARY = 3 };
 
 struct KeySet {
     KeyCol col[MAX_KEYS];
@@ -229,13 +230,17 @@ __device__ __forceinline__ uint64_t row_hash(const KeySet& ks, int64_t row, cons
         if (c.validity && !bit_is_set(c.validity, j)) continue;
         uint64_t v;
         if (c.mode == KEY_HASH_DICTIONARY) {
-            int64_t idx;
+            uint64_t raw;
             switch (c.width) {
-                case 8: idx = ((const int64_t*)c.values)[j]; break;
-                case 4: idx = ((const int32_t*)c.values)[j]; break;
-                case 2: idx = ((const int16_t*)c.values)[j]; break;
-                default: idx = ((const int8_t*)c.values)[j]; break;
+                case 8: raw = ((const uint64_t*)c.values)[j]; break;
+                case 4: raw = ((const uint32_t*)c.values)[j]; break;
+                case 2: raw = ((const uint16_t*)c.values)[j]; break;
+                default: raw = ((const uint8_t*)c.values)[j]; break;
             }
+            // zero-extended load, then a shift pair sign-extends signed indices (this form leaves the generic scatter kernels'
+            // registers and spills as they were with signed loads); 8-byte indices are taken as they are: a valid one is below 2^63
+            const unsigned s = c.index_unsigned ? 0u : 64u - 8u * (unsigned)c.width;
+            const int64_t idx = (int64_t)(raw << s) >> s;
             if (c.dict_validity && !bit_is_set(c.dict_validity, idx)) continue;
             v = ((const uint64_t*)c.offsets)[idx];
         } else {

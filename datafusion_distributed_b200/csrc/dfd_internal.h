@@ -55,7 +55,7 @@ struct dfd_partitioner {
     uint32_t N = 0;
     std::vector<int32_t> key_cols;
     std::vector<int32_t> key_modes;  // dfd_key_hash_mode per key column
-    struct KeyDict { const uint64_t* hashes = nullptr; const uint8_t* validity = nullptr; };
+    struct KeyDict { const uint64_t* hashes = nullptr; const uint8_t* validity = nullptr; bool index_unsigned = false; };
     std::vector<KeyDict> key_dicts;  // DFD_KEY_HASH_DICTIONARY: device hashes / validity of the dictionary values
     dfd::HashState st{};
     dfd::ModN mod{};
@@ -137,7 +137,12 @@ int launch_scatter_onepass_peer(const ScatterParams& sp, int width, bool fast, i
 int launch_scatter_follow_local(const ScatterParams& sp, int width, bool fast, int sm_count, size_t smem, cudaStream_t stream);
 int launch_scatter_follow_peer(const ScatterParams& sp, int width, bool fast, int sm_count, size_t smem, cudaStream_t stream);
 
-// create_hashes over device columns -> raw u64 row hashes (dictionary values, parity hook).  Caller holds ctx->mu.
+// Column kinds that only the host operator hands to hash_columns_locked, never part of the C ABI: Interval(DayTime) (8 bytes)
+// and Interval(MonthDayNano) (16 bytes) dictionary VALUES, hashed field by field like interval keys (KEY_HASH_INTERVAL_*).
+constexpr int32_t COL_INTERVAL_DAY_TIME = 5, COL_INTERVAL_MONTH_DAY_NANO = 6;
+
+// create_hashes over device columns -> raw u64 row hashes (dictionary values, parity hook).  Besides the DFD_COL_* kinds a
+// column may be COL_INTERVAL_DAY_TIME / COL_INTERVAL_MONTH_DAY_NANO.  Caller holds ctx->mu.
 int hash_columns_locked(Ctx* c, const dfd_column* cols, int n_cols, int64_t n_rows, const uint64_t* seeds, uint64_t* hashes_device, cudaStream_t stream);
 
 // Launches K1 -> K1b -> K2 on `stream`; caller holds ctx->mu and has set the device.

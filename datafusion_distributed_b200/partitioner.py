@@ -51,21 +51,27 @@ class HashPartitioner:
         """Interval(DayTime) / Interval(MonthDayNano) keys hash field by field (`dfd_partitioner_set_key_hash_mode`)."""
         nv.check(nv.lib().dfd_partitioner_set_key_hash_mode(self._h, key_index, mode))
 
-    def set_key_dictionary(self, key_index: int, dictionary_values):
+    def set_key_dictionary(self, key_index: int, dictionary_values, unsigned_index: bool = False):
         """Key column `key_index` holds dictionary INDICES of `dictionary_values` (a pyarrow Array, or None to make the key
         plain again): hash the values once on the device (`dfd_hash_columns_device`) and let rows take
-        dict_hashes[index] (`dfd_partitioner_set_key_dictionary`) — DataFusion's hash_dictionary."""
+        dict_hashes[index] (`dfd_partitioner_set_key_dictionary`) — DataFusion's hash_dictionary.  `unsigned_index`:
+        the indices are UInt8/16/32/64 (read zero-extended) rather than Int8/16/32/64."""
         if not hasattr(self, "_dicts"):
             self._dicts = {}
         if dictionary_values is None:
-            nv.check(nv.lib().dfd_partitioner_set_key_dictionary(self._h, key_index, None, None))
+            nv.check(nv.lib().dfd_partitioner_set_key_dictionary(self._h, key_index, None, None, 0))
             self._dicts.pop(key_index, None)
             return
+        import pyarrow as pa
+
+        if pa.types.is_interval(dictionary_values.type):  # dfd_hash_columns_device would hash them as one integer
+            raise ValueError(f"dictionary values of type {dictionary_values.type} cannot be a partitioner key here: intervals hash field "
+                             "by field (RepartitionExec handles Dictionary<_, Interval> keys)")
         vals = DeviceColumn.from_arrow(self.ctx, dictionary_values)
         n = len(dictionary_values)
         hashes = self.ctx.alloc(max(n * 8, 8))
         nv.check(nv.lib().dfd_hash_columns_device(self.ctx.handle, columns_to_c([vals]), 1, n, None, hashes.ptr))
-        nv.check(nv.lib().dfd_partitioner_set_key_dictionary(self._h, key_index, hashes.ptr, vals.validity or None))
+        nv.check(nv.lib().dfd_partitioner_set_key_dictionary(self._h, key_index, hashes.ptr, vals.validity or None, int(bool(unsigned_index))))
         self._dicts[key_index] = (vals, hashes)  # keep the device buffers alive
 
     @property

@@ -152,15 +152,20 @@ int dfd_partitioner_set_key_hash_mode(dfd_partitioner* p, int key_index, int mod
 /* Dictionary-encoded key columns (Arrow Dictionary<K, V>; the reference's bench schema has Dictionary<Int32, Utf8>,
  * src/execution_plans/benchmarks/fixture.rs:13-33).  DataFusion's hash_dictionary hashes the dictionary VALUES once
  * (create_hashes over the values array) and every row takes dict_hashes[index]; a null index or a null dictionary value
- * leaves the running hash untouched.  Pass the INDICES as the (fixed-width, signed) key column and declare its dictionary
- * here: dict_hashes_device = the values' hashes (dfd_hash_columns_device over the values column, asynchronous on the
- * context's stream), dict_validity_device = the values' validity bitmap or NULL.  The pointers must stay valid while
- * partition calls use them; NULL hashes turn the key back into a plain one.  As PAYLOAD the indices are a plain
- * fixed-width column and the dictionary travels by reference (host operator) — see dfd_repartition_exec. */
+ * leaves the running hash untouched.  Pass the INDICES as the (fixed-width, 1/2/4/8-byte) key column and declare its
+ * dictionary here: dict_hashes_device = the values' hashes (dfd_hash_columns_device over the values column, asynchronous
+ * on the context's stream), dict_validity_device = the values' validity bitmap or NULL, index_is_unsigned = nonzero for
+ * UInt8/16/32/64 indices (zero-extended; 0: Int8/16/32/64, sign-extended).  The pointers must stay valid while partition
+ * calls use them; NULL hashes turn the key back into a plain one.  Interval(DayTime) / Interval(MonthDayNano) VALUES cannot
+ * be hashed through dfd_hash_columns_device (see there).  As PAYLOAD the indices are a plain fixed-width column and the
+ * dictionary travels by reference (host operator) — see dfd_repartition_exec, which handles every index type and
+ * interval values itself. */
 int dfd_partitioner_set_key_dictionary(dfd_partitioner* p, int key_index, const uint64_t* dict_hashes_device,
-                                       const uint8_t* dict_validity_device);
+                                       const uint8_t* dict_validity_device, int index_is_unsigned);
 /* hashes_device[i] = create_hashes(cols, RandomState::with_seeds(seeds or 0,0,0,0))[i] — raw 64-bit row hashes
- * (null rows of a single column hash to 0).  Asynchronous on dfd_ctx_stream(). */
+ * (null rows of a single column hash to 0).  Asynchronous on dfd_ctx_stream().  Every FIXED column hashes as one integer:
+ * Interval(DayTime) / Interval(MonthDayNano) columns are NOT hashed field by field here as DataFusion does (that needs a
+ * partitioner with dfd_partitioner_set_key_hash_mode). */
 int dfd_hash_columns_device(dfd_ctx* ctx, const dfd_column* cols, int n_cols, int64_t n_rows, const uint64_t* seeds,
                             uint64_t* hashes_device);
 

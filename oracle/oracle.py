@@ -157,13 +157,18 @@ class _Cols:
     def _fill(self, d: OrcColumn, col):
         import pyarrow as pa
 
-        if isinstance(col, tuple):  # ("interval_day_time" | "interval_month_day_nano", raw little-endian values as a uint8 array)
-            tag, raw = col
+        if isinstance(col, tuple):
+            # ("interval_day_time" | "interval_month_day_nano", raw little-endian values as a uint8 array[, valid: bool per row])
+            tag, raw, *valid = col
             raw = np.ascontiguousarray(raw, dtype=np.uint8)
             self.keep.append(raw)
             d.kind = ORC_INTERVAL_DAY_TIME if tag == "interval_day_time" else ORC_INTERVAL_MONTH_DAY_NANO
             d.width = 8 if tag == "interval_day_time" else 16
             d.values, d.offsets, d.validity, d.offset = raw.ctypes.data, None, None, 0
+            if valid and valid[0] is not None:
+                bits = np.packbits(np.asarray(valid[0], dtype=bool), bitorder="little")
+                self.keep.append(bits)
+                d.validity = bits.ctypes.data
             return
         if isinstance(col, np.ndarray):
             col = np.ascontiguousarray(col)

@@ -94,7 +94,10 @@ int dfd::hash_columns_locked(Ctx*, const dfd_column* cols, int n_cols, int64_t n
     KernelTime kernel_time;
     if (!cols || n_cols < 1 || n_rows < 0 || !hashes_device) return set_error(DFD_ERR_INVALID_ARGUMENT, "hash_columns: bad arguments");
     std::vector<orc_column> oc;
-    for (int i = 0; i < n_cols; ++i) oc.push_back(to_orc(cols[i], DFD_KEY_HASH_PLAIN));
+    for (int i = 0; i < n_cols; ++i)  // (the operator's interval dictionary values arrive as the internal interval kinds)
+        oc.push_back(to_orc(cols[i], cols[i].kind == dfd::COL_INTERVAL_DAY_TIME         ? DFD_KEY_HASH_INTERVAL_DAY_TIME
+                                     : cols[i].kind == dfd::COL_INTERVAL_MONTH_DAY_NANO ? DFD_KEY_HASH_INTERVAL_MONTH_DAY_NANO
+                                                                                        : DFD_KEY_HASH_PLAIN));
     const orc_random_state st = state_of(seeds);
     memset(hashes_device, 0, sizeof(uint64_t) * (size_t)n_rows);
     orc_create_hashes(oc.data(), n_cols, n_rows, &st, hashes_device);
@@ -125,9 +128,9 @@ int harness_destinations(dfd_partitioner* p, const dfd_column* in, int n_cols, i
                 int64_t idx;
                 switch (c.width) {
                     case 8: idx = ((const int64_t*)c.values)[j]; break;
-                    case 4: idx = ((const int32_t*)c.values)[j]; break;
-                    case 2: idx = ((const int16_t*)c.values)[j]; break;
-                    default: idx = ((const int8_t*)c.values)[j]; break;
+                    case 4: idx = d.index_unsigned ? (int64_t)((const uint32_t*)c.values)[j] : ((const int32_t*)c.values)[j]; break;
+                    case 2: idx = d.index_unsigned ? (int64_t)((const uint16_t*)c.values)[j] : ((const int16_t*)c.values)[j]; break;
+                    default: idx = d.index_unsigned ? (int64_t)((const uint8_t*)c.values)[j] : ((const int8_t*)c.values)[j]; break;
                 }
                 if (d.validity && !bit(d.validity, idx)) continue;
                 h[(size_t)i] = k >= 1 ? orc_combine_hashes(d.hashes[idx], h[(size_t)i]) : d.hashes[idx];

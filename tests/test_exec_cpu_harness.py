@@ -189,6 +189,23 @@ def test_host_logic_of_the_operator_against_the_oracle(harness, monkeypatch, nam
         assert ctx.lib.harness_kernel_launches(ctx.handle) > before  # the operator really ran through the stand-in partitioner
 
 
+def _key_cases():
+    from tests import test_exec_keys_gpu as K
+
+    return K.HARNESS_CASES
+
+
+@pytest.mark.parametrize("body,args", _key_cases(), ids=[f"{b}-{'-'.join(map(str, a))}" for b, a in _key_cases()])
+def test_key_types_through_the_operator_against_the_oracle(harness, monkeypatch, body, args):
+    """The bodies of tests/test_exec_keys_gpu.py (every key format, every Dictionary<K, V> key, unsigned indices past the
+    signed range) with the operator's host logic on the stand-in partitioner."""
+    from tests import test_exec_keys_gpu as K
+
+    _, ctx = harness
+    monkeypatch.setattr(K, "native", lambda: ctx.lib)
+    getattr(K, body)(ctx, *args)
+
+
 def test_the_product_package_never_loads_the_harness():
     """The harness is test infrastructure: nothing under the product package or the bench refers to it."""
     for top in ("datafusion_distributed_b200", "bench.py", "bench_workloads.py", "__graft_entry__.py"):
