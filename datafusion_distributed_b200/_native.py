@@ -140,6 +140,7 @@ SIGNATURES = {
                                               C.POINTER(DfdExecOptions), C.POINTER(_VP)]),
     "dfd_repartition_exec_destroy": (None, [_VP]),
     "dfd_repartition_exec_push": (C.c_int, [_VP, C.POINTER(ArrowArrayStruct)]),
+    "dfd_repartition_exec_push_device": (C.c_int, [_VP, C.POINTER(ArrowDeviceArrayStruct)]),
     "dfd_repartition_exec_finish": (C.c_int, [_VP]),
     "dfd_repartition_exec_abort": (C.c_int, [_VP, C.c_char_p]),
     "dfd_repartition_exec_run": (C.c_int, [_VP, C.POINTER(ArrowArrayStreamStruct)]),

@@ -462,7 +462,10 @@ struct Slot {
     OutChunk* out = nullptr;
     bool in_flight = false;
     std::vector<HeldInput> held;
+    std::vector<HeldInput> dict_held;  // device input: host copies of the dictionaries of the batches in `held` (what the output references)
 };
+
+enum InputMode { INPUT_UNSET = 0, INPUT_HOST = 1, INPUT_DEVICE = 2 };
 
 }  // namespace
 
@@ -496,6 +499,13 @@ struct dfd_repartition_exec {
     // host scratch of the batch being staged (pageable: an H2D from it has been staged by the time cudaMemcpyAsync returns)
     std::vector<std::vector<char>> tmp_off, tmp_bytes;
     std::vector<VarPrep> prep;
+    // device input (push_device): the first non-empty push decides whether the operator takes host or device batches
+    int input_mode = INPUT_UNSET;
+    dfd::Scratch d_sizes;                  // k_stage_sizes results, 4 x int64 per var-width column
+    int64_t* h_sizes = nullptr;            // pinned: their read-back
+    cudaEvent_t e_sizes = nullptr;
+    std::vector<dfd::Scratch> view_tmp;    // view fields: [lengths | offsets | scan block sums | data buffer table] (device)
+    std::vector<std::vector<int64_t>> dsz; // per visible field: the read-back sizes of the rows being staged
 };
 
 namespace {
@@ -535,9 +545,10 @@ int emit_slot(dfd_repartition_exec* x, Slot& s) {
         x->ns_wait_d2h += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count();
     }
     OutChunk* oc = s.out;
-    for (const FieldInfo& f : x->fields)
-        if (f.dict) { oc->inputs = s.held; break; }  // the output batches reference the inputs' dictionaries
+    for (const FieldInfo& f : x->fields)  // the output batches reference the inputs' dictionaries (device input: their host copies)
+        if (f.dict) { oc->inputs = x->input_mode == INPUT_DEVICE ? s.dict_held : s.held; break; }
     s.held.clear();
+    s.dict_held.clear();
     s.out = nullptr;
     s.in_flight = false;
     const size_t C = x->n_visible;  // the output batches carry the schema's columns; hidden list columns are folded into their list
@@ -669,6 +680,7 @@ int flush_current(dfd_repartition_exec* x) {
     std::lock_guard<std::mutex> lk(c->mu);
     XCUDA(x, cudaSetDevice(c->device), "cudaSetDevice");
     for (int fi : x->dev_fields) {  // the buffers concatenated on the host while staging: bitmaps and re-based offsets
+        if (x->input_mode == INPUT_DEVICE) break;  // (device input: k_stage_batch built them in place)
         const size_t i = (size_t)fi;
         const FieldInfo& f = x->fields[i];
         const size_t bm = (size_t)((s.rows + 7) / 8);
@@ -810,6 +822,9 @@ DictId dict_identity(const ArrowArray* d) {
     return DictId{d->n_buffers > 0 ? d->buffers[d->n_buffers - 1] : nullptr, d->offset, d->length};
 }
 
+bool same_dictionary(const FieldInfo& f, const ArrowArray* mine, const ArrowArray* theirs);
+int grow_var_bytes(dfd_repartition_exec* x, int64_t n, bool* fits);
+
 // Host-side preparation of rows [start, start + n) of `b` for the open chunk: where every variable-width device column's
 // offsets and bytes come from (views and lists are converted to offsets + bytes here, index arithmetic only), and whether
 // these rows can JOIN the chunk (`*fits`): same dictionaries, and string bytes within the offset width.  The chunk's
@@ -890,18 +905,28 @@ int prepare_rows(dfd_repartition_exec* x, const ArrowArray* b, int64_t start, in
             const DictId id = dict_identity(c->dictionary);
             if (s.rows > 0 && !(s.dict_id[i] == id)) {
                 const ArrowArray* mine = !s.held.empty() && s.held.front()->array.children[i] ? s.held.front()->array.children[i]->dictionary : nullptr;
-                const ArrowArray* theirs = c->dictionary;
-                const bool dvar = f.dict_kind == DFD_COL_UTF8 || f.dict_kind == DFD_COL_LARGE_UTF8 || f.dict_kind == DFD_COL_BINARY;
-                const bool comparable = mine && f.dict_format[0] != 'v' && mine->length == theirs->length && mine->n_buffers == theirs->n_buffers &&
-                                        mine->length <= (1 << 16);  // (a linear comparison per batch: only worth it for small dictionaries — a batch's own)
-                if (!comparable || !dfd::host::flat_arrays_equal(mine->length, dvar ? (f.dict_kind == DFD_COL_LARGE_UTF8 ? 8 : 4) : 0,
-                                                                  f.dict_kind == DFD_COL_BOOL ? 0 : f.dict_width, mine->buffers, mine->offset, mine->null_count,
-                                                                  theirs->buffers, theirs->offset, theirs->null_count))
-                    *fits = false;
+                if (!same_dictionary(f, mine, c->dictionary)) *fits = false;
             }
         }
     }
     if (!*fits) return DFD_OK;
+    return grow_var_bytes(x, n, fits);
+}
+
+// Does a dictionary with other buffers (`theirs`) hold the same values as the chunk's (`mine`)?  Both in host memory.
+bool same_dictionary(const FieldInfo& f, const ArrowArray* mine, const ArrowArray* theirs) {
+    const bool dvar = f.dict_kind == DFD_COL_UTF8 || f.dict_kind == DFD_COL_LARGE_UTF8 || f.dict_kind == DFD_COL_BINARY;
+    const bool comparable = mine && f.dict_format[0] != 'v' && mine->length == theirs->length && mine->n_buffers == theirs->n_buffers &&
+                            mine->length <= (1 << 16);  // (a linear comparison per batch: only worth it for small dictionaries — a batch's own)
+    return comparable && dfd::host::flat_arrays_equal(mine->length, dvar ? (f.dict_kind == DFD_COL_LARGE_UTF8 ? 8 : 4) : 0,
+                                                      f.dict_kind == DFD_COL_BOOL ? 0 : f.dict_width, mine->buffers, mine->offset, mine->null_count,
+                                                      theirs->buffers, theirs->offset, theirs->null_count);
+}
+
+// The string bytes `x->prep` says rows [.., + n) add: cut the chunk early (`*fits` = false) when they would pass what 32-bit
+// offsets address, otherwise grow the chunk's byte buffers when they need more room.
+int grow_var_bytes(dfd_repartition_exec* x, int64_t n, bool* fits) {
+    Slot& s = x->slots[x->cur];
     for (int fi : x->dev_fields) {
         const size_t h = (size_t)fi;
         const FieldInfo& f = x->fields[h];
@@ -1062,6 +1087,382 @@ int emit_ready(dfd_repartition_exec* x) {
         if (rc) return rc;
     }
     return DFD_OK;
+}
+
+// ---- device input (dfd_repartition_exec_push_device): the same chunks, assembled on the device by k_stage_* ---------------
+
+// the host waits for everything enqueued on the staging stream so far (read-backs of sizes / dictionaries)
+int wait_staging(dfd_repartition_exec* x) {
+    {
+        std::lock_guard<std::mutex> lk(x->ctx->mu);
+        XCUDA(x, cudaSetDevice(x->ctx->device), "cudaSetDevice");
+        if (!x->e_sizes) XCUDA(x, cudaEventCreateWithFlags(&x->e_sizes, cudaEventDisableTiming), "cudaEventCreate");
+        XCUDA(x, cudaEventRecord(x->e_sizes, x->s_h2d), "record read-back");
+    }
+    XCUDA(x, cudaEventSynchronize(x->e_sizes), "read-back");
+    return DFD_OK;
+}
+
+// Host copies of the dictionaries of one device batch.  The output batches are host arrays and reference these (held by
+// the chunk), so a device batch need not outlive the device work that reads it.
+struct HostDicts {
+    std::vector<ArrowArray> kids;  // per column: only `dictionary` is set
+    std::vector<ArrowArray*> kid_ptrs;
+    std::vector<ArrowArray> dicts;
+    std::vector<std::vector<const void*>> bufs;
+    std::vector<std::vector<char>> mem;
+};
+void host_dicts_release(ArrowArray* a) {
+    delete (HostDicts*)a->private_data;
+    a->release = nullptr;
+}
+
+int host_dictionaries(dfd_repartition_exec* x, const ArrowArray* b, HeldInput* out) {
+    const size_t C = x->n_visible;
+    std::unique_ptr<HostDicts> h(new HostDicts());
+    h->kids.resize(C);
+    h->kid_ptrs.resize(C);
+    h->dicts.resize(C);
+    h->bufs.resize(C);
+    for (size_t i = 0; i < C; ++i) {
+        memset(&h->kids[i], 0, sizeof(ArrowArray));
+        h->kids[i].release = child_release;
+        h->kid_ptrs[i] = &h->kids[i];
+    }
+    auto copy = [&](const void* src, size_t n) -> const void* {  // D2H on the staging stream (after the producer's event)
+        h->mem.emplace_back(n + 8);
+        char* dst = h->mem.back().data();
+        if (n && cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, x->s_h2d) != cudaSuccess) return nullptr;
+        x->bytes_d2h += n;
+        return dst;
+    };
+    for (int phase = 0; phase < 2; ++phase) {  // 0: validity, values, offsets, views, variadic sizes; 1: the bytes they locate
+        {
+            std::lock_guard<std::mutex> lk(x->ctx->mu);
+            XCUDA(x, cudaSetDevice(x->ctx->device), "cudaSetDevice");
+            for (size_t i = 0; i < C; ++i) {
+                const FieldInfo& f = x->fields[i];
+                const ArrowArray* d = f.dict ? b->children[i]->dictionary : nullptr;
+                if (!d) continue;  // (prepare refuses a dictionary column without a dictionary)
+                const int64_t dn = d->offset + d->length;
+                const bool view = f.dict_format[0] == 'v';
+                const bool dvar = !view && (f.dict_kind == DFD_COL_UTF8 || f.dict_kind == DFD_COL_LARGE_UTF8 || f.dict_kind == DFD_COL_BINARY);
+                const size_t dow = f.dict_kind == DFD_COL_LARGE_UTF8 ? 8 : 4;
+                std::vector<const void*>& hb = h->bufs[i];
+                bool ok = true;
+                if (phase == 0) {
+                    if (d->n_buffers < (view ? 3 : dvar ? 3 : 2) || !d->buffers || !d->buffers[1])
+                        return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": malformed dictionary");
+                    hb.assign((size_t)d->n_buffers, nullptr);
+                    if (d->null_count != 0 && d->buffers[0]) ok &= (hb[0] = copy(d->buffers[0], (size_t)((dn + 7) / 8))) != nullptr;
+                    const size_t nb1 = f.dict_kind == DFD_COL_BOOL ? (size_t)((dn + 7) / 8) : view ? (size_t)dn * 16 : dvar ? (size_t)(dn + 1) * dow : (size_t)dn * f.dict_width;
+                    ok &= (hb[1] = copy(d->buffers[1], nb1)) != nullptr;
+                    if (view) ok &= (hb[(size_t)d->n_buffers - 1] = copy(d->buffers[d->n_buffers - 1], (size_t)(d->n_buffers - 3) * 8)) != nullptr;
+                } else if (dvar) {
+                    const int64_t last = dow == 8 ? ((const int64_t*)hb[1])[dn] : ((const int32_t*)hb[1])[dn];
+                    ok &= (hb[2] = copy(d->buffers[2], (size_t)(last > 0 ? last : 0))) != nullptr;
+                } else if (view) {
+                    const int64_t* sizes = (const int64_t*)hb[(size_t)d->n_buffers - 1];
+                    for (int64_t k = 0; k + 3 < d->n_buffers; ++k) ok &= (hb[(size_t)k + 2] = copy(d->buffers[k + 2], (size_t)sizes[k])) != nullptr;
+                }
+                if (!ok) return fail(x, DFD_ERR_CUDA, "column " + f.name + ": D2H of the dictionary failed");
+            }
+        }
+        if (int rc = wait_staging(x)) return rc;
+    }
+    for (size_t i = 0; i < C; ++i) {
+        const ArrowArray* d = x->fields[i].dict ? b->children[i]->dictionary : nullptr;
+        if (!d) continue;
+        ArrowArray& hd = h->dicts[i];
+        hd = *d;
+        hd.buffers = h->bufs[i].data();
+        hd.n_children = 0;
+        hd.children = nullptr;
+        hd.dictionary = nullptr;
+        hd.release = child_release;
+        hd.private_data = nullptr;
+        h->kids[i].dictionary = &hd;
+    }
+    ArrowArray top;
+    memset(&top, 0, sizeof top);
+    top.length = b->length;
+    top.n_children = (int64_t)C;
+    top.children = h->kid_ptrs.data();
+    top.release = host_dicts_release;
+    top.private_data = h.release();
+    *out = std::make_shared<SharedInput>(top);
+    return DFD_OK;
+}
+
+struct ViewTmp {  // byte offsets of the parts of a view field's device scratch, for n rows and `nbuf` variadic buffers
+    size_t lens, off, sums, ptrs, total;
+    ViewTmp(int64_t n, int64_t nbuf) {
+        auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
+        lens = 0;
+        off = al((size_t)n * 4 + 16);
+        sums = off + al((size_t)(n + 1) * 4 + 16);
+        ptrs = sums + al((size_t)(n / 2048 + 4) * 8);
+        total = ptrs + al((size_t)(nbuf > 0 ? nbuf : 1) * 8);
+    }
+};
+
+// Device counterpart of prepare_rows: the same checks and chunk cuts.  Variable-width columns need their byte counts on
+// the host (buffer growth, the 2 GiB cut of 32-bit offsets, values_bytes): k_stage_sizes computes them for all such
+// columns at once, and the host reads them back (one small D2H and one wait; never for fixed-width-only schemas).
+int prepare_rows_device(dfd_repartition_exec* x, const ArrowArray* b, const HeldInput& dicts, int64_t start, int64_t n, bool* fits) {
+    Slot& s = x->slots[x->cur];
+    *fits = true;
+    std::vector<StageSize> jobs;
+    std::vector<size_t> job_field;
+    for (size_t i = 0; i < x->n_visible; ++i) {
+        const FieldInfo& f = x->fields[i];
+        const ArrowArray* c = b->children[i];
+        const int64_t lo = c->offset + start;
+        if (validity_of(c) && !(f.flags & ARROW_FLAG_NULLABLE) && c->null_count > 0)
+            return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": nulls in a column the schema declares non-nullable");
+        StageSize j;
+        j.lo = lo;
+        j.n = n;
+        if (f.list) {
+            if (c->n_children != 1 || !c->children[0]) return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": list array without a child");
+            const ArrowArray* v = c->children[0];
+            j.op = STAGE_SIZE_LIST;
+            j.off = c->buffers[1];
+            j.off2 = f.child_width > 0 ? nullptr : (const int32_t*)v->buffers[1] + v->offset;
+        } else if (f.var() && f.view) {
+            j.op = STAGE_SIZE_VIEW;  // (j.lens: set once the field's scratch is sized, below)
+            j.off = c->buffers[1];
+            j.valid = validity_of(c);
+        } else if (f.var()) {
+            j.op = STAGE_SIZE_RANGE;
+            j.ow = (int32_t)f.ow();
+            j.off = c->buffers[1];
+        } else {
+            if (f.dict) {
+                if (!c->dictionary) return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": dictionary array without a dictionary");
+                const DictId id = dict_identity(c->dictionary);  // (identity of the DEVICE dictionary; values compared on the host copies)
+                if (s.rows > 0 && !(s.dict_id[i] == id)) {
+                    const ArrowArray* mine = !s.dict_held.empty() ? s.dict_held.front()->array.children[i]->dictionary : nullptr;
+                    if (!same_dictionary(f, mine, dicts->array.children[i]->dictionary)) *fits = false;
+                }
+            }
+            continue;
+        }
+        jobs.push_back(j);
+        job_field.push_back(i);
+    }
+    if (!*fits || jobs.empty()) return DFD_OK;
+    const size_t nb = jobs.size() * 4 * sizeof(int64_t);
+    {
+        std::lock_guard<std::mutex> lk(x->ctx->mu);
+        XCUDA(x, cudaSetDevice(x->ctx->device), "cudaSetDevice");
+        if (int rc = x->d_sizes.ensure(nb, x->ctx->device)) return fail(x, rc, dfd_last_error());
+        if (!x->h_sizes) XCUDA(x, cudaHostAlloc((void**)&x->h_sizes, x->fields.size() * 4 * sizeof(int64_t), cudaHostAllocPortable), "cudaHostAlloc(sizes)");
+        for (size_t k = 0; k < jobs.size(); ++k) {
+            jobs[k].out = (int64_t*)x->d_sizes.ptr + 4 * k;
+            if (jobs[k].op != STAGE_SIZE_VIEW) continue;
+            const ViewTmp vt(n, b->children[job_field[k]]->n_buffers - 3);
+            if (int rc = x->view_tmp[job_field[k]].ensure(vt.total, x->ctx->device)) return fail(x, rc, dfd_last_error());
+            jobs[k].lens = (int32_t*)((char*)x->view_tmp[job_field[k]].ptr + vt.lens);
+        }
+        XCUDA(x, cudaMemsetAsync(x->d_sizes.ptr, 0, nb, x->s_h2d), "memset sizes");
+        int rc = launch_stage_sizes(jobs.data(), (int)jobs.size(), x->s_h2d);
+        for (size_t k = 0; k < jobs.size() && !rc; ++k) {  // views: offsets = exclusive scan of the lengths
+            if (jobs[k].op != STAGE_SIZE_VIEW) continue;
+            const ViewTmp vt(n, b->children[job_field[k]]->n_buffers - 3);
+            char* t = (char*)x->view_tmp[job_field[k]].ptr;
+            rc = launch_lengths_to_offsets(t + vt.lens, 4, n, (unsigned long long*)(t + vt.sums), t + vt.off, x->s_h2d);
+        }
+        if (rc) return fail(x, rc, dfd_last_error());
+        XCUDA(x, cudaMemcpyAsync(x->h_sizes, x->d_sizes.ptr, nb, cudaMemcpyDeviceToHost, x->s_h2d), "D2H sizes");
+    }
+    if (int rc = wait_staging(x)) return rc;
+    for (size_t k = 0; k < jobs.size(); ++k) {
+        const size_t i = job_field[k];
+        const FieldInfo& f = x->fields[i];
+        const int64_t* r = x->h_sizes + 4 * k;
+        x->dsz[i].assign(r, r + 4);
+        if (f.list) {
+            const int64_t ne = r[1] - r[0], cw = f.child_width;
+            if (ne < 0 || (cw == 0 && r[3] < r[2])) return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": list offsets are not monotonic");
+            if (ne * 4 > 0x7fffffffLL || ne * (cw > 0 ? cw : 1) > 0x7fffffffLL)
+                return fail(x, DFD_ERR_UNSUPPORTED, "column " + f.name + ": too many list elements in one chunk");
+            x->prep[(size_t)f.h_len].nbytes = ne * 4;
+            x->prep[(size_t)f.h_bytes].nbytes = cw > 0 ? ne * cw : r[3] - r[2];
+            if (f.h_valid >= 0) x->prep[(size_t)f.h_valid].nbytes = ne;
+        } else if (f.view) {
+            if (r[0] > 0x7fffffffLL) return fail(x, DFD_ERR_UNSUPPORTED, "column " + f.name + ": more than 2 GiB of view data in one chunk");
+            x->prep[i].nbytes = r[0];
+        } else {
+            if (r[1] < r[0]) return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": offsets are not monotonic");
+            x->prep[i].first = r[0];
+            x->prep[i].nbytes = r[1] - r[0];
+        }
+    }
+    return grow_var_bytes(x, n, fits);
+}
+
+// Device counterpart of stage_rows: append rows [start, start + n) of the device batch `b` to the open chunk — every buffer
+// of every column in ONE k_stage_batch launch (plus a small H2D of the data buffer table of each view column).
+int stage_rows_device(dfd_repartition_exec* x, const ArrowArray* b, const HeldInput& dicts, int64_t start, int64_t n) {
+    Slot& s = x->slots[x->cur];
+    std::lock_guard<std::mutex> lk(x->ctx->mu);
+    XCUDA(x, cudaSetDevice(x->ctx->device), "cudaSetDevice");
+    std::vector<StageJob> jobs;
+    auto validity = [&](size_t i, const uint8_t* valid, int64_t lo) {
+        if (!valid && !s.has_valid[i]) return;
+        StageJob j;
+        j.op = STAGE_BITS;
+        j.src = valid;
+        j.a = lo;
+        j.dst = s.d_in_valid[i];
+        j.b = s.rows;
+        j.c = s.has_valid[i] ? s.rows : 0;  // the first batch with a validity bitmap: earlier rows of the chunk count as valid
+        j.n = n;
+        s.has_valid[i] = true;
+        jobs.push_back(j);
+    };
+    auto offsets = [&](size_t h, const void* src, int ow_in, int64_t scale) {
+        StageJob j;
+        j.op = STAGE_OFFSETS;
+        j.src = src;
+        j.ow_in = ow_in;
+        j.ow_out = (int32_t)x->fields[h].ow();
+        j.dst = (char*)s.d_in_off[h] + (size_t)s.rows * x->fields[h].ow();
+        j.n = n;
+        j.base = s.data_bytes[h];
+        j.scale = scale;
+        return j;
+    };
+    auto bytes = [&](size_t h, StageJob j) {  // (after the column's offsets job, which takes the old byte count as its base)
+        j.dst = (char*)s.d_in[h] + s.data_bytes[h];
+        jobs.push_back(j);
+        s.data_bytes[h] += x->prep[h].nbytes;
+    };
+    for (size_t i = 0; i < x->n_visible; ++i) {
+        const FieldInfo& f = x->fields[i];
+        const ArrowArray* c = b->children[i];
+        const int64_t lo = c->offset + start;
+        const uint8_t* valid = (f.flags & ARROW_FLAG_NULLABLE) ? validity_of(c) : nullptr;
+        if (f.list) {
+            const ArrowArray* v = c->children[0];
+            const size_t hl = (size_t)f.h_len, hb = (size_t)f.h_bytes;
+            const int32_t* loff = (const int32_t*)c->buffers[1] + lo;
+            const int32_t* coff = f.child_width > 0 ? nullptr : (const int32_t*)v->buffers[1] + v->offset;
+            const int64_t e0 = x->dsz[i][0], ne = x->dsz[i][1] - e0, cw = f.child_width;
+            jobs.push_back(offsets(hl, loff, 4, 4));
+            StageJob len;
+            if (cw > 0) { len.op = STAGE_FILL32; len.base = cw; }
+            else { len.op = STAGE_DIFF32; len.src = coff + e0; }
+            len.n = ne;
+            bytes(hl, len);
+            if (cw > 0) {
+                jobs.push_back(offsets(hb, loff, 4, cw));
+            } else {
+                StageJob lo_ = offsets(hb, loff, 4, 1);
+                lo_.op = STAGE_LIST_OFFSETS;
+                lo_.src2 = coff;
+                jobs.push_back(lo_);
+            }
+            StageJob cp;
+            cp.src = cw > 0 ? (const char*)v->buffers[1] + (size_t)(v->offset + e0) * (size_t)cw : (const char*)v->buffers[2] + x->dsz[i][2];
+            cp.n = x->prep[hb].nbytes;
+            bytes(hb, cp);
+            if (f.h_valid >= 0) {
+                const size_t hv = (size_t)f.h_valid;
+                jobs.push_back(offsets(hv, loff, 4, 1));
+                StageJob vb;
+                vb.op = STAGE_BIT_BYTES;
+                vb.src = validity_of(v);
+                vb.a = v->offset + e0;
+                vb.n = ne;
+                bytes(hv, vb);
+            }
+            validity(hl, valid, lo);  // the list's own validity rides on the lengths column
+            continue;
+        }
+        if (f.dict && s.rows == 0) s.dict_id[i] = dict_identity(c->dictionary);
+        if (f.dict && x->key_of_field[i] >= 0 && s.rows == 0) {
+            // dictionary KEY: hash the device-resident values in place once per chunk (DataFusion hash_dictionary)
+            const ArrowArray* d = c->dictionary;
+            const ArrowArray* hd = dicts->array.children[i]->dictionary;  // (host copy: the byte count of string values)
+            const int64_t dn = d->offset + d->length;
+            const bool dvar = f.dict_kind == DFD_COL_UTF8 || f.dict_kind == DFD_COL_LARGE_UTF8 || f.dict_kind == DFD_COL_BINARY;
+            const bool dhv = d->null_count != 0 && d->n_buffers > 0 && d->buffers[0] != nullptr;
+            int64_t dbytes = 0;
+            if (dvar) dbytes = f.dict_kind == DFD_COL_LARGE_UTF8 ? ((const int64_t*)hd->buffers[1])[dn] : ((const int32_t*)hd->buffers[1])[dn];
+            const size_t vbytes = f.dict_kind == DFD_COL_BOOL ? (size_t)((dn + 7) / 8) : (dvar ? (size_t)dbytes : (size_t)dn * f.dict_width);
+            int rc = s.dict_buf[i].ensure((size_t)(d->length + 1) * 8, x->ctx->device);
+            if (rc) return fail(x, rc, dfd_last_error());
+            const int32_t dmode = interval_key_mode(f.dict_format);
+            const int32_t hkind = dmode == DFD_KEY_HASH_INTERVAL_DAY_TIME ? COL_INTERVAL_DAY_TIME
+                                  : dmode == DFD_KEY_HASH_INTERVAL_MONTH_DAY_NANO ? COL_INTERVAL_MONTH_DAY_NANO : f.dict_kind;
+            dfd_column dc{hkind, f.dict_width, (void*)d->buffers[dvar ? 2 : 1], dvar ? (void*)d->buffers[1] : nullptr, dhv ? (uint8_t*)d->buffers[0] : nullptr,
+                          d->offset, (int64_t)vbytes};
+            rc = hash_columns_locked(x->ctx, &dc, 1, d->length, nullptr, (uint64_t*)s.dict_buf[i].ptr, x->s_h2d);
+            if (rc) return fail(x, rc, dfd_last_error());
+            s.dict_hashes[i] = (const uint64_t*)s.dict_buf[i].ptr;
+            s.dict_valid[i] = dhv ? (const uint8_t*)d->buffers[0] : nullptr;  // (the first batch of the chunk stays held until its D2H is done)
+            if (dhv && d->offset != 0) return fail(x, DFD_ERR_UNSUPPORTED, "column " + f.name + ": sliced dictionary values with nulls are not supported yet");
+        }
+        if (f.var() && f.view) {
+            // Utf8View / BinaryView: lengths and their scan came with the sizes; the data buffer table goes to the device
+            const int64_t nbuf = c->n_buffers - 3;  // (validity, views, data buffers..., variadic sizes: the sizes are not read)
+            const ViewTmp vt(n, nbuf);
+            char* t = (char*)x->view_tmp[i].ptr;
+            if (nbuf > 0)
+                XCUDA(x, cudaMemcpyAsync(t + vt.ptrs, c->buffers + 2, (size_t)nbuf * sizeof(void*), cudaMemcpyHostToDevice, x->s_h2d), "H2D view buffer table");
+            jobs.push_back(offsets(i, t + vt.off, 4, 1));
+            StageJob vb;
+            vb.op = STAGE_VIEW_BYTES;
+            vb.src = (const uint8_t*)c->buffers[1] + (size_t)lo * 16;
+            vb.src2 = t + vt.ptrs;
+            vb.src3 = t + vt.off;
+            vb.n = n;
+            bytes(i, vb);
+        } else if (f.var()) {
+            jobs.push_back(offsets(i, (const char*)c->buffers[1] + (size_t)lo * f.ow(), (int)f.ow(), 1));
+            StageJob cp;
+            cp.src = (const char*)c->buffers[2] + x->prep[i].first;
+            cp.n = x->prep[i].nbytes;
+            bytes(i, cp);
+        } else if (f.kind == DFD_COL_FIXED) {
+            StageJob cp;
+            cp.src = (const char*)c->buffers[1] + (size_t)lo * f.width;
+            cp.dst = (char*)s.d_in[i] + (size_t)s.rows * f.width;
+            cp.n = n * f.width;
+            jobs.push_back(cp);
+        } else {  // boolean values: one more bitmap
+            StageJob bv;
+            bv.op = STAGE_BITS;
+            bv.src = c->buffers[1];
+            bv.a = lo;
+            bv.dst = s.d_in[i];
+            bv.b = bv.c = s.rows;
+            bv.n = n;
+            jobs.push_back(bv);
+        }
+        validity(i, valid, lo);
+    }
+    if (int rc = launch_stage_batch(jobs.data(), (int)jobs.size(), x->s_h2d)) return fail(x, rc, dfd_last_error());
+    s.rows += n;
+    return DFD_OK;
+}
+
+// After an error or an abort of a device-input operator: wait for the device work that still reads the pushed batches,
+// then release them (the producer gets its memory back now, not when the operator is destroyed).
+void release_device_inputs(dfd_repartition_exec* x) {
+    {
+        std::lock_guard<std::mutex> lk(x->ctx->mu);
+        cudaSetDevice(x->ctx->device);
+        cudaStreamSynchronize(x->s_h2d);
+        cudaStreamSynchronize(x->ctx->stream);
+        cudaStreamSynchronize(x->s_d2h);
+    }
+    for (Slot& s : x->slots) {
+        s.held.clear();
+        s.dict_held.clear();
+    }
 }
 
 }  // namespace
@@ -1318,6 +1719,8 @@ int dfd_repartition_exec_create(dfd_ctx* ctx, const struct ArrowSchema* schema, 
     x->tmp_off.resize(x->fields.size());
     x->tmp_bytes.resize(x->fields.size());
     x->prep.resize(x->fields.size());
+    x->view_tmp.resize(x->fields.size());
+    x->dsz.assign(x->fields.size(), std::vector<int64_t>(4, 0));
     x->cur = x->depth - 1;  // open_next_slot() starts at slot 0
     *out = x.release();
     return DFD_OK;
@@ -1331,8 +1734,13 @@ void dfd_repartition_exec_destroy(dfd_repartition_exec* x) {
         if (x->s_h2d) cudaStreamSynchronize(x->s_h2d);
         if (x->s_d2h) cudaStreamSynchronize(x->s_d2h);
         cudaStreamSynchronize(x->ctx->stream);
+        cudaFree(x->d_sizes.ptr);
+        for (dfd::Scratch& b : x->view_tmp) cudaFree(b.ptr);
+        if (x->h_sizes) cudaFreeHost(x->h_sizes);
+        if (x->e_sizes) cudaEventDestroy(x->e_sizes);
         for (Slot& s : x->slots) {
             s.held.clear();
+            s.dict_held.clear();
             if (s.out) { s.out->refs.store(1); s.out->pool = x->pool; chunk_unref(s.out); }
             for (void* p : s.d_in) cudaFree(p);
             for (void* p : s.d_in_valid) cudaFree(p);
@@ -1372,11 +1780,18 @@ int dfd_repartition_exec_push(dfd_repartition_exec* x, struct ArrowArray* batch)
     const int64_t R = batch->length;
     x->rows_in += (uint64_t)R;
     if (R == 0) { drop(); return DFD_OK; }
+    if (x->input_mode == INPUT_DEVICE) {
+        drop();
+        const int rc = fail(x, DFD_ERR_INVALID_ARGUMENT, "host batch pushed to an operator that takes device batches (push_device)");
+        release_device_inputs(x);
+        return rc;
+    }
     for (int64_t i = 0; i < batch->n_children; ++i)
         if (batch->children[i]->length < R || (batch->offset != 0)) {
             drop();
             return fail(x, DFD_ERR_INVALID_ARGUMENT, "record batch children shorter than the batch, or non-zero struct offset");
         }
+    x->input_mode = INPUT_HOST;
     // ownership of the batch moves to a shared holder: every chunk that stages rows from it (and, for dictionary columns,
     // every output batch that references its dictionaries) keeps it alive
     HeldInput holder = std::make_shared<SharedInput>(*batch);
@@ -1410,6 +1825,85 @@ int dfd_repartition_exec_push(dfd_repartition_exec* x, struct ArrowArray* batch)
     return emit_ready(x);
 }
 
+int dfd_repartition_exec_push_device(dfd_repartition_exec* x, struct ArrowDeviceArray* batch) {
+    if (!x || !batch) return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_repartition_exec_push_device: NULL argument");
+    ScopedNs timed(x->ns_push);
+    ArrowArray* a = &batch->array;
+    auto drop = [&]() { if (a->release) a->release(a); };
+    if (x->finished) { drop(); return set_error(DFD_ERR_INVALID_ARGUMENT, "push after finish/error: %s", x->error.c_str()); }
+    auto refuse = [&](int code, const std::string& msg) {  // the batch is released, the operator fails (and lets go of earlier batches)
+        drop();
+        const int rc = fail(x, code, msg);
+        if (x->input_mode == INPUT_DEVICE) release_device_inputs(x);
+        return rc;
+    };
+    if (!launch_stage_batch || !launch_stage_sizes)  // (weak: see dfd_internal.h)
+        return refuse(DFD_ERR_UNSUPPORTED, "device input: this build of the operator has no staging kernels (dfd_stage.cu)");
+    if (batch->device_type != ARROW_DEVICE_CUDA || batch->device_id != (int64_t)x->ctx->device)
+        return refuse(DFD_ERR_INVALID_ARGUMENT, "device batch of device type " + std::to_string((int)batch->device_type) + ", device " +
+                                                    std::to_string(batch->device_id) + ": the operator takes CUDA batches of device " +
+                                                    std::to_string(x->ctx->device));
+    if (a->n_children != (int64_t)x->n_visible)
+        return refuse(DFD_ERR_INVALID_ARGUMENT, "batch has " + std::to_string(a->n_children) + " columns, schema has " + std::to_string(x->n_visible));
+    const int64_t R = a->length;
+    x->rows_in += (uint64_t)R;
+    if (R == 0) { drop(); return DFD_OK; }
+    if (x->input_mode == INPUT_HOST)
+        return refuse(DFD_ERR_INVALID_ARGUMENT, "device batch pushed to an operator that takes host batches (push / run)");
+    for (int64_t i = 0; i < a->n_children; ++i)
+        if (a->children[i]->length < R || (a->offset != 0))
+            return refuse(DFD_ERR_INVALID_ARGUMENT, "record batch children shorter than the batch, or non-zero struct offset");
+    x->input_mode = INPUT_DEVICE;
+    if (batch->sync_event) {  // the staging stream waits for the producer's work; the host does not
+        cudaError_t e;
+        {
+            std::lock_guard<std::mutex> lk(x->ctx->mu);
+            e = cudaSetDevice(x->ctx->device);
+            if (e == cudaSuccess) e = cudaStreamWaitEvent(x->s_h2d, *(cudaEvent_t*)batch->sync_event, 0);
+        }
+        if (e != cudaSuccess) return refuse(DFD_ERR_CUDA, std::string("wait on the batch's sync_event: ") + cudaGetErrorString(e));
+    }
+    // ownership moves to a shared holder, as in push(): released once the chunks that read it have been emitted
+    HeldInput holder = std::make_shared<SharedInput>(*a);
+    a->release = nullptr;
+    const ArrowArray* in = &holder->array;
+    auto bail = [&](int rc) {
+        release_device_inputs(x);
+        return rc;
+    };
+    int rc = DFD_OK;
+    HeldInput dicts;
+    for (const FieldInfo& f : x->fields)
+        if (f.dict) {
+            if ((rc = host_dictionaries(x, in, &dicts))) return bail(rc);
+            break;
+        }
+    int64_t done = 0;
+    while (done < R) {
+        if (!x->cur_open && (rc = open_next_slot(x))) return bail(rc);
+        Slot& s = x->slots[x->cur];
+        const int64_t room = x->chunk_rows - s.rows;
+        if (room == 0) {
+            if ((rc = flush_current(x))) return bail(rc);
+            continue;
+        }
+        const int64_t n = R - done < room ? R - done : room;
+        bool fits = true;
+        if ((rc = prepare_rows_device(x, in, dicts, done, n, &fits))) return bail(rc);
+        if (!fits) {
+            if ((rc = flush_current(x))) return bail(rc);
+            continue;
+        }
+        if ((rc = stage_rows_device(x, in, dicts, done, n))) return bail(rc);
+        s.held.push_back(holder);
+        if (dicts) s.dict_held.push_back(dicts);
+        done += n;
+        if (s.rows == x->chunk_rows && (rc = flush_current(x))) return bail(rc);
+    }
+    if ((rc = emit_ready(x))) return bail(rc);
+    return DFD_OK;
+}
+
 int dfd_repartition_exec_finish(dfd_repartition_exec* x) {
     if (!x) return set_error(DFD_ERR_INVALID_ARGUMENT, "NULL exec");
     if (x->finished) return x->error_code ? set_error(x->error_code, "%s", x->error.c_str()) : DFD_OK;
@@ -1432,6 +1926,7 @@ int dfd_repartition_exec_abort(dfd_repartition_exec* x, const char* message) {
     if (!x) return set_error(DFD_ERR_INVALID_ARGUMENT, "NULL exec");
     if (x->finished) return DFD_OK;  // already finished or failed: the first outcome stands
     fail(x, DFD_ERR_INTERNAL, std::string("aborted by the producer: ") + (message ? message : "input failed"));
+    if (x->input_mode == INPUT_DEVICE) release_device_inputs(x);
     return DFD_OK;
 }
 

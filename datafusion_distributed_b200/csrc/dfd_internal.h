@@ -127,6 +127,50 @@ int launch_offsets_to_lengths(const void* off, int ow, int64_t n, void* len, cud
 int launch_var_dest_bytes(const void* off, int ow, const int64_t* part_starts, uint32_t N, int64_t* bytes, int64_t* first, cudaStream_t s);
 int launch_lengths_to_offsets(const void* len, int ow, int64_t n, unsigned long long* block_sums /*[n/2048 + 2]*/, void* out_off, cudaStream_t s);
 
+// Device-side chunk assembly for device-resident input batches (dfd_repartition_exec_push_device; kernels in dfd_stage.cu).
+// One StageJob appends one buffer of one column to the open chunk; all jobs of a pushed batch go out in one launch
+// (STAGE_MAX_JOBS per launch, as a __grid_constant__ table).  Offsets are re-based as dst[r] = base + scale * (src[r] - src[0]).
+enum StageOp : int32_t {
+    STAGE_COPY = 0,      // dst[0, n) = src[0, n) (bytes)
+    STAGE_BITS = 1,      // bitmap append: dst bits [c, b) = 1, dst bits [b, b + n) = src bits [a, a + n) (src NULL: all ones)
+    STAGE_OFFSETS = 2,   // dst[r] = base + scale * (src[r] - src[0]), r in [0, n]; ow_in / ow_out = 4 or 8 bytes
+    STAGE_LIST_OFFSETS = 3,  // list child bytes: dst[r] = base + src2[src[r]] - src2[src[0]], r in [0, n] (int32 list + child offsets)
+    STAGE_DIFF32 = 4,    // element lengths: dst[k] = src[k + 1] - src[k], k < n (int32)
+    STAGE_FILL32 = 5,    // dst[k] = (int32) base, k < n
+    STAGE_BIT_BYTES = 6, // dst[k] = bit a + k of src (src NULL: 1), one byte each, k < n
+    STAGE_VIEW_BYTES = 7,  // 16-byte views src[0, n) -> bytes at dst + src3[r] (src3 = int32 offsets, src2 = data buffer table)
+};
+struct StageJob {
+    int32_t op = STAGE_COPY, ow_in = 4, ow_out = 4, pad = 0;
+    const void* src = nullptr;
+    const void* src2 = nullptr;
+    const void* src3 = nullptr;
+    void* dst = nullptr;
+    int64_t n = 0, a = 0, b = 0, c = 0, base = 0, scale = 1;
+};
+constexpr int STAGE_MAX_JOBS = 32;
+// The two staging launches are WEAK references of the operator object: it also links without dfd_stage.cu (a build of the
+// operator's host logic on its own, with no device code), and push_device then refuses device batches with an error —
+// never a fallback.  libdfd_b200.so always links dfd_stage.cu, so there both are defined.
+__attribute__((weak)) int launch_stage_batch(const StageJob* jobs, int n_jobs, cudaStream_t s);
+
+// What the host must know of a var-width column before it stages rows [lo, lo + n): read back once per pushed batch.
+enum StageSizeOp : int32_t {
+    STAGE_SIZE_RANGE = 0,  // out[0] = off[lo], out[1] = off[lo + n] (ow = 4 or 8)
+    STAGE_SIZE_LIST = 1,   // out[0] = e0 = off[lo], out[1] = e1 = off[lo + n]; with off2 (child offsets): out[2] = off2[e0], out[3] = off2[e1]
+    STAGE_SIZE_VIEW = 2,   // lens[r] = length of view lo + r (0 when null), out[0] += sum of lens (caller zeroes out)
+};
+struct StageSize {
+    int32_t op = STAGE_SIZE_RANGE, ow = 4;
+    const void* off = nullptr;
+    const void* off2 = nullptr;
+    const uint8_t* valid = nullptr;
+    int64_t lo = 0, n = 0;
+    int32_t* lens = nullptr;
+    int64_t* out = nullptr;  // 4 values
+};
+__attribute__((weak)) int launch_stage_sizes(const StageSize* jobs, int n_jobs, cudaStream_t s);
+
 // Aligned write-out (k_scatter KV > K) is used for the peer-store exchange at small N (full-size NVLink write packets).
 bool use_aligned(uint32_t N, bool peer);
 // Kernel launch dispatch, one translation unit each (dfd_scatter_*.cu, templates in dfd_launch.cuh)

@@ -98,6 +98,13 @@ class RepartitionExec:
         batch._export_to_c(C.addressof(ca))
         nv.check(nv.lib().dfd_repartition_exec_push(self._h, C.byref(ca)))
 
+    def push_device_batch(self, device_array):
+        """Feed one DEVICE-resident input batch: a pointer (int or ctypes) to a `struct ArrowDeviceArray` on this worker's
+        GPU.  Ownership of its `array` moves to the operator (its release is called once the device work that reads it is
+        done).  An operator takes either host batches (`push_batch` / `run`) or device batches, never both."""
+        addr = device_array if isinstance(device_array, int) else C.addressof(device_array)
+        nv.check(nv.lib().dfd_repartition_exec_push_device(self._h, C.cast(C.c_void_p(addr), C.POINTER(nv.ArrowDeviceArrayStruct))))
+
     def finish(self):
         nv.check(nv.lib().dfd_repartition_exec_finish(self._h))
 

@@ -315,6 +315,28 @@ int dfd_repartition_exec_create(dfd_ctx* ctx, const struct ArrowSchema* schema, 
                                 dfd_repartition_exec** out);
 void dfd_repartition_exec_destroy(dfd_repartition_exec* x);
 int dfd_repartition_exec_push(dfd_repartition_exec* x, struct ArrowArray* batch);
+/* A DEVICE-resident record batch (Arrow C Device Data Interface), for producers whose data is already on the GPU: no
+ * input byte crosses PCIe and nothing is staged on the host; the chunk is assembled on the device.
+ *   - batch->device_type == ARROW_DEVICE_CUDA and batch->device_id == the context's device; anything else (CPU,
+ *     CUDA_HOST, managed memory, another GPU) is refused with DFD_ERR_INVALID_ARGUMENT.  Every buffer of the struct
+ *     array, its children, their dictionaries and list children is in that GPU's memory; the ArrowArray structs and
+ *     their `buffers` pointer arrays are in host memory (as the C Device interface specifies).
+ *   - sync_event: NULL or a cudaEvent_t*.  The operator's staging stream waits on it (cudaStreamWaitEvent) before
+ *     reading anything; the host does not block on it.
+ *   - Ownership of batch->array moves to the operator, as with push: its release is called exactly once, after the
+ *     device work that reads it has completed — at finish() at the latest, and on every error path (and abort).
+ *   - Accepted schemas, batch shapes and rules are those of push (same column count, children at least as long as the
+ *     batch, struct offset 0, sliced children, null_count 0 / -1 / n, batches of any length, malformed input refused).
+ *   - An operator takes either host batches (push / run) or device batches: the first non-empty push decides, and a
+ *     push of the other kind releases its batch and fails the operator with DFD_ERR_INVALID_ARGUMENT.
+ *   - The partition streams are identical to those push() gives for the same batch contents (batches and their
+ *     boundaries, row order, values incl. the bytes under null slots, validity, offsets, views, dictionaries, lists).
+ *     Output batches are host arrays; a dictionary column references a HOST copy of the dictionary values.
+ *   - dfd_exec_stats: rows_in counts the rows, bytes_h2d stays 0, dictionaries copied to the host count in bytes_d2h.
+ *     Schemas with variable-width, view or list columns read each batch's byte counts back (one small D2H and one
+ *     wait per batch); fixed-width / boolean / dictionary-index-only schemas never wait for the device while pushing,
+ *     except to copy dictionaries to the host. */
+int dfd_repartition_exec_push_device(dfd_repartition_exec* x, struct ArrowDeviceArray* batch);
 int dfd_repartition_exec_finish(dfd_repartition_exec* x);
 /* The producer's INPUT failed: instead of finish(), fail the operator — every partition stream's get_next returns EIO
  * with `message` (rows already queued are still delivered first), exactly as RepartitionExec forwards an input error

@@ -3,7 +3,7 @@
 //! (`include/arrow_c_abi.h` is the same layout).
 #![allow(non_camel_case_types)]
 
-use std::ffi::{c_char, c_int};
+use std::ffi::{c_char, c_int, c_void};
 
 use arrow::ffi::{FFI_ArrowArray, FFI_ArrowSchema};
 use arrow::ffi_stream::FFI_ArrowArrayStream;
@@ -44,6 +44,18 @@ pub struct dfd_exec_stats {
     pub ns_wait_pool: u64,
 }
 
+/// `struct ArrowDeviceArray` of the Arrow C Device Data Interface (`include/arrow_c_abi.h`): a record batch whose buffers
+/// live on a GPU; `sync_event` is NULL or a `cudaEvent_t*`.
+#[repr(C)]
+pub struct ArrowDeviceArray {
+    pub array: FFI_ArrowArray,
+    pub device_id: i64,
+    pub device_type: i32,
+    pub sync_event: *mut c_void,
+    pub reserved: [i64; 3],
+}
+pub const ARROW_DEVICE_CUDA: i32 = 2;
+
 // dfd_status (include/dfd_b200.h)
 pub const DFD_OK: c_int = 0;
 pub const DFD_ERR_INVALID_ARGUMENT: c_int = 1;
@@ -74,6 +86,9 @@ extern "C" {
     ) -> c_int;
     /// One input `RecordBatch`; ownership of `*batch` moves to the operator (its `release` is cleared). Single producer.
     pub fn dfd_repartition_exec_push(x: *mut dfd_repartition_exec, batch: *mut FFI_ArrowArray) -> c_int;
+    /// One GPU-resident input batch (same device as the context); ownership of `batch.array` moves to the operator. An
+    /// operator takes either host batches (`push`) or device batches, decided by the first non-empty push.
+    pub fn dfd_repartition_exec_push_device(x: *mut dfd_repartition_exec, batch: *mut ArrowDeviceArray) -> c_int;
     pub fn dfd_repartition_exec_finish(x: *mut dfd_repartition_exec) -> c_int;
     /// The input failed: every partition stream ends with EIO + `message` (RepartitionExec forwards input errors likewise).
     pub fn dfd_repartition_exec_abort(x: *mut dfd_repartition_exec, message: *const c_char) -> c_int;
