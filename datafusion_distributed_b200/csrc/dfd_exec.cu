@@ -46,7 +46,7 @@ struct FieldInfo {
     // After the scatter the child offsets are an exclusive scan of the gathered lengths and the child validity is re-packed.
     bool list = false, hidden = false;
     int h_len = -1, h_bytes = -1, h_valid = -1;
-    int owner = -1, role = 0;  // hidden columns: the list field they belong to; role 1 = lengths, 2 = bytes, 3 = element validity
+    int role = 0;  // hidden columns: 1 = lengths, 2 = bytes, 3 = element validity
     std::string child_name, child_format;
     int64_t child_flags = 0;
     int32_t child_width = 0;       // list child: 0 = Utf8 / Binary (offsets + bytes), > 0 = fixed-width primitive of that many bytes
@@ -56,8 +56,12 @@ struct FieldInfo {
     std::string dict_format;
     int64_t dict_flags = 0;
     int32_t dict_kind = DFD_COL_FIXED, dict_width = 0;
-    bool var() const { return kind == DFD_COL_UTF8 || kind == DFD_COL_LARGE_UTF8 || kind == DFD_COL_BINARY; }
+    static bool var_kind(int32_t k) { return k == DFD_COL_UTF8 || k == DFD_COL_LARGE_UTF8 || k == DFD_COL_BINARY; }
+    bool var() const { return var_kind(kind); }
     size_t ow() const { return kind == DFD_COL_LARGE_UTF8 ? 8 : 4; }  // offset width of var-width kinds
+    bool dict_var() const { return var_kind(dict_kind); }             // dictionary values with offsets + bytes
+    size_t dict_ow() const { return dict_kind == DFD_COL_LARGE_UTF8 ? 8 : 4; }
+    int32_t dict_hash_kind() const;                                    // how the device hashes the dictionary values
 };
 
 // LargeBinary and FixedSizeBinary values are hashed by DataFusion as byte slices with a length prefix; the device hashes a
@@ -68,6 +72,11 @@ bool hashable_format(const char* f) { return f[0] != 'Z' && f[0] != 'w'; }
 // a dictionary key alike; everything else is one integer / byte-slice write.
 int32_t interval_key_mode(const std::string& f) {
     return f == "tiD" ? DFD_KEY_HASH_INTERVAL_DAY_TIME : f == "tin" ? DFD_KEY_HASH_INTERVAL_MONTH_DAY_NANO : DFD_KEY_HASH_PLAIN;
+}
+
+int32_t FieldInfo::dict_hash_kind() const {
+    const int32_t mode = interval_key_mode(dict_format);
+    return mode == DFD_KEY_HASH_INTERVAL_DAY_TIME ? COL_INTERVAL_DAY_TIME : mode == DFD_KEY_HASH_INTERVAL_MONTH_DAY_NANO ? COL_INTERVAL_MONTH_DAY_NANO : dict_kind;
 }
 
 // Arrow format string -> physical layout (Arrow C data interface, "Data type description")
@@ -427,11 +436,21 @@ struct PartQueue {
 
 using HeldInput = std::shared_ptr<SharedInput>;  // an input batch whose buffers an in-flight H2D still reads
 
-struct VarPrep {  // rows of one variable-width device column as they will be staged: n + 1 source offsets (the first being
-    const char* off = nullptr;   // `first`) and the bytes they span
-    int64_t first = 0;
-    const char* bytes = nullptr;
+struct VarPrep {  // rows of one variable-width device column as they will be staged: the first source offset and the
+    int64_t first = 0;  // byte count (lists and views are staged from zero-based offsets built for them)
     int64_t nbytes = 0;
+};
+
+struct Span {  // what rows [lo, lo + n) of a visible variable-width field span in its buffers
+    int64_t first = 0, last = 0;              // offsets at lo and lo + n (lists: element offsets; views: 0 and the byte total)
+    int64_t child_first = 0, child_last = 0;  // lists of strings: the child offsets at those elements
+};
+
+struct FieldTmp {  // per field: the rows being staged
+    std::vector<char> off, bytes;  // host input: offsets / bytes built for a view field or a hidden list column
+    VarPrep prep;                  // variable-width device columns
+    Span span;                     // visible variable-width and list fields
+    dfd::Scratch view_dev;         // view fields, device input: [lengths | offsets | scan block sums | data buffer table]
 };
 
 struct DictId {  // identity of a dictionary: values buffer, offset, length
@@ -440,29 +459,34 @@ struct DictId {  // identity of a dictionary: values buffer, offset, length
     bool operator==(const DictId& o) const { return p == o.p && offset == o.offset && length == o.length; }
 };
 
+struct SlotCol {  // one field of a slot
+    void *d_in = nullptr, *d_in_valid = nullptr, *d_out = nullptr, *d_out_valid = nullptr;  // device buffers
+    void *d_in_off = nullptr, *d_out_off = nullptr;  // var-width: offsets buffers
+    size_t in_cap = 0, out_cap = 0;                  // var-width: capacity of d_in / d_out (string bytes)
+    int64_t data_bytes = 0;                          // var-width: byte count of the chunk
+    uint8_t *h_valid = nullptr, *h_bool = nullptr;   // pinned, allocated on first use: the chunk's validity / boolean bitmaps,
+                                                     //   concatenated on the host at bit granularity (bit r = row r of the chunk)
+    char* h_off = nullptr;                           // pinned: the chunk's var-width offsets, re-based onto the chunk's byte buffer
+    bool has_valid = false;
+    DictId dict_id;                                  // dictionary fields: identity of the chunk's dictionary
+    dfd::Scratch list_tmp;                           // list fields: [child offsets | child validity bits | scan block sums] (device)
+    dfd::Scratch dict_buf;                           // dictionary KEY fields: [hashes | offsets | data | validity] of the values
+    const uint64_t* dict_hashes = nullptr;           //   device pointers handed to the partitioner for this chunk
+    const uint8_t* dict_valid = nullptr;
+};
+
 struct Slot {
-    std::vector<void*> d_in, d_in_valid, d_out, d_out_valid;  // per column device buffers
-    std::vector<void*> d_in_off, d_out_off;                   // var-width: offsets buffers
-    std::vector<size_t> in_cap, out_cap;                      // var-width: capacity of d_in / d_out (string bytes)
-    std::vector<int64_t> first_off, data_bytes;               // var-width: first input offset / byte count of the chunk
-    std::vector<uint8_t*> h_valid, h_bool;                    // pinned, allocated on first use: the chunk's validity / boolean bitmaps,
-                                                              //   concatenated on the host at bit granularity (bit r = row r of the chunk)
-    std::vector<char*> h_off;                                 // pinned: the chunk's var-width offsets, re-based onto the chunk's byte buffer
-    std::vector<DictId> dict_id;                              // dictionary columns: identity of the chunk's dictionary
-    std::vector<dfd::Scratch> list_tmp;                       // list fields: [child offsets | child validity bits | scan block sums] (device)
-    std::vector<dfd::Scratch> dict_buf;                       // dictionary KEY columns: [hashes | offsets | data | validity] of the values
-    std::vector<const uint64_t*> dict_hashes;                 //   device pointers handed to the partitioner for this chunk
-    std::vector<const uint8_t*> dict_valid;
-    int64_t* h_part_starts = nullptr;                        // pinned [N+1]
+    std::vector<SlotCol> col;  // per field
+    int64_t* h_part_starts = nullptr;  // pinned [N+1]
     cudaEvent_t e_h2d = nullptr, e_k = nullptr, e_d2h = nullptr;
     bool k_recorded = false, d2h_recorded = false;
     // state of the chunk currently in this slot
     int64_t rows = 0;
-    std::vector<bool> has_valid;
     OutChunk* out = nullptr;
     bool in_flight = false;
     std::vector<HeldInput> held;
-    std::vector<HeldInput> dict_held;  // device input: host copies of the dictionaries of the batches in `held` (what the output references)
+    std::vector<HeldInput> dict_held;  // what the output batches' dictionaries reference: the batches in `held` (host input)
+                                       //   or host copies of their dictionaries (device input); empty without dictionary fields
 };
 
 enum InputMode { INPUT_UNSET = 0, INPUT_HOST = 1, INPUT_DEVICE = 2 };
@@ -475,8 +499,7 @@ struct dfd_repartition_exec {
     std::vector<FieldInfo> fields;
     std::vector<int> key_of_field;  // index into the partitioner's key list, or -1
     size_t n_visible = 0;           // fields [0, n_visible) are the schema's columns; the rest are hidden device columns (lists)
-    std::vector<int> dev_fields;    // fields that own a device column, in launch order; dev_pos[field] = its position there
-    std::vector<int> dev_pos;
+    std::vector<int> dev_fields;    // fields that own a device column, in launch order
     uint32_t N = 0;
     int64_t chunk_rows = 0;
     int depth = 3;
@@ -496,16 +519,14 @@ struct dfd_repartition_exec {
     std::atomic<uint64_t> rows_in{0}, bytes_h2d{0}, bytes_d2h{0};
     uint64_t rows_out = 0;  // (under `mu`)
     std::atomic<uint64_t> ns_push{0}, ns_wait_d2h{0}, ns_wait_pool{0};  // producer-thread time: inside push/finish; of which blocked on a D2H / on the pinned pool
-    // host scratch of the batch being staged (pageable: an H2D from it has been staged by the time cudaMemcpyAsync returns)
-    std::vector<std::vector<char>> tmp_off, tmp_bytes;
-    std::vector<VarPrep> prep;
-    // device input (push_device): the first non-empty push decides whether the operator takes host or device batches
+    // per field: the batch being staged (host memory is pageable: an H2D from it has been staged by the time
+    // cudaMemcpyAsync returns)
+    std::vector<FieldTmp> tmp;
+    // the first non-empty push decides whether the operator takes host (push) or device (push_device) batches
     int input_mode = INPUT_UNSET;
-    dfd::Scratch d_sizes;                  // k_stage_sizes results, 4 x int64 per var-width column
+    dfd::Scratch d_sizes;                  // device input: k_stage_sizes results, 4 x int64 per var-width column
     int64_t* h_sizes = nullptr;            // pinned: their read-back
     cudaEvent_t e_sizes = nullptr;
-    std::vector<dfd::Scratch> view_tmp;    // view fields: [lengths | offsets | scan block sums | data buffer table] (device)
-    std::vector<std::vector<int64_t>> dsz; // per visible field: the read-back sizes of the rows being staged
 };
 
 namespace {
@@ -540,19 +561,16 @@ int fail(dfd_repartition_exec* x, int code, const std::string& msg) {
 int emit_slot(dfd_repartition_exec* x, Slot& s) {
     if (!s.in_flight) return DFD_OK;
     {
-        const auto t0 = std::chrono::steady_clock::now();
+        ScopedNs waited(x->ns_wait_d2h);
         XCUDA(x, cudaEventSynchronize(s.e_d2h), "D2H");
-        x->ns_wait_d2h += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count();
     }
     OutChunk* oc = s.out;
-    for (const FieldInfo& f : x->fields)  // the output batches reference the inputs' dictionaries (device input: their host copies)
-        if (f.dict) { oc->inputs = x->input_mode == INPUT_DEVICE ? s.dict_held : s.held; break; }
+    oc->inputs = std::move(s.dict_held);  // the output batches reference the inputs' dictionaries
     s.held.clear();
     s.dict_held.clear();
     s.out = nullptr;
     s.in_flight = false;
     const size_t C = x->n_visible;  // the output batches carry the schema's columns; hidden list columns are folded into their list
-    int made = 0;
     for (size_t c = 0; c < C; ++c) {
         if (!x->fields[c].list) continue;
         int32_t* lo32 = (int32_t*)oc->offsets[(size_t)x->fields[c].h_len];  // byte offsets into the 4-byte lengths -> element offsets
@@ -584,12 +602,12 @@ int emit_slot(dfd_repartition_exec* x, Slot& s) {
         for (size_t c = 0; c < C; ++c) {
             ArrowArray& a = bp->children[c];
             memset(&a, 0, sizeof a);
-            bool hv = s.has_valid[c];
+            bool hv = s.col[c].has_valid;
             const FieldInfo& f = x->fields[c];
             if (f.list) {
                 // List<Utf8>: list offsets + validity from the lengths column, values array (offsets from the device scan, bytes, validity)
                 const size_t hl = (size_t)f.h_len, hb = (size_t)f.h_bytes;
-                const bool lv = s.has_valid[hl];
+                const bool lv = s.col[hl].has_valid;
                 bp->child_bufs[4 * c] = lv ? oc->validity[hl] : nullptr;
                 bp->child_bufs[4 * c + 1] = oc->offsets[hl];
                 ArrowArray& g = bp->grand[c];
@@ -597,7 +615,7 @@ int emit_slot(dfd_repartition_exec* x, Slot& s) {
                 bp->grand_bufs[3 * c] = f.h_valid >= 0 ? oc->values[(size_t)f.h_valid] : nullptr;
                 bp->grand_bufs[3 * c + 1] = f.child_width > 0 ? oc->values[hb] : oc->values[hl];  // primitive child: [validity, values]
                 bp->grand_bufs[3 * c + 2] = oc->values[hb];
-                g.length = s.data_bytes[hl] / 4;
+                g.length = s.col[hl].data_bytes / 4;
                 g.null_count = f.h_valid >= 0 ? -1 : 0;
                 g.n_buffers = f.child_width > 0 ? 2 : 3;
                 g.buffers = &bp->grand_bufs[3 * c];
@@ -647,7 +665,6 @@ int emit_slot(dfd_repartition_exec* x, Slot& s) {
         top.release = batch_release;
         top.private_data = bp;
         oc->refs.fetch_add(1);
-        ++made;
         {
             std::lock_guard<std::mutex> lk(x->mu);
             x->queues[p].batches.push_back(top);
@@ -655,7 +672,6 @@ int emit_slot(dfd_repartition_exec* x, Slot& s) {
         }
     }
     chunk_unref(oc);  // drop the guard (returns the chunk to the pool if nothing was emitted)
-    (void)made;
     x->cv.notify_all();
     return DFD_OK;
 }
@@ -672,28 +688,27 @@ int flush_current(dfd_repartition_exec* x) {
     // the producer waits for a consumer to release a chunk (back-pressure), and other operators of the same worker context
     // must keep running meanwhile
     {
-        const auto t0 = std::chrono::steady_clock::now();
+        ScopedNs waited(x->ns_wait_pool);
         s.out = x->pool->acquire();
-        x->ns_wait_pool += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count();
     }
     if (!s.out) return fail(x, DFD_ERR_OOM, "pinned host allocation failed");
     std::lock_guard<std::mutex> lk(c->mu);
     XCUDA(x, cudaSetDevice(c->device), "cudaSetDevice");
     for (int fi : x->dev_fields) {  // the buffers concatenated on the host while staging: bitmaps and re-based offsets
         if (x->input_mode == INPUT_DEVICE) break;  // (device input: k_stage_batch built them in place)
-        const size_t i = (size_t)fi;
-        const FieldInfo& f = x->fields[i];
+        const FieldInfo& f = x->fields[(size_t)fi];
+        SlotCol& sc = s.col[(size_t)fi];
         const size_t bm = (size_t)((s.rows + 7) / 8);
-        if (s.has_valid[i]) {
-            XCUDA(x, cudaMemcpyAsync(s.d_in_valid[i], s.h_valid[i], bm, cudaMemcpyHostToDevice, x->s_h2d), "H2D validity");
+        if (sc.has_valid) {
+            XCUDA(x, cudaMemcpyAsync(sc.d_in_valid, sc.h_valid, bm, cudaMemcpyHostToDevice, x->s_h2d), "H2D validity");
             x->bytes_h2d += bm;
         }
         if (f.kind == DFD_COL_BOOL) {
-            XCUDA(x, cudaMemcpyAsync(s.d_in[i], s.h_bool[i], bm, cudaMemcpyHostToDevice, x->s_h2d), "H2D boolean values");
+            XCUDA(x, cudaMemcpyAsync(sc.d_in, sc.h_bool, bm, cudaMemcpyHostToDevice, x->s_h2d), "H2D boolean values");
             x->bytes_h2d += bm;
         }
         if (f.var()) {
-            XCUDA(x, cudaMemcpyAsync(s.d_in_off[i], s.h_off[i], (size_t)(s.rows + 1) * f.ow(), cudaMemcpyHostToDevice, x->s_h2d), "H2D offsets");
+            XCUDA(x, cudaMemcpyAsync(sc.d_in_off, sc.h_off, (size_t)(s.rows + 1) * f.ow(), cudaMemcpyHostToDevice, x->s_h2d), "H2D offsets");
             x->bytes_h2d += (size_t)(s.rows + 1) * f.ow();
         }
     }
@@ -703,24 +718,24 @@ int flush_current(dfd_repartition_exec* x) {
     const size_t D = x->dev_fields.size();  // device columns: every field except the list placeholders (+ the hidden list columns)
     std::vector<dfd_column> in(D), out(D);
     for (size_t k = 0; k < D; ++k) {
-        const size_t i = (size_t)x->dev_fields[k];
-        const FieldInfo& f = x->fields[i];
+        const FieldInfo& f = x->fields[(size_t)x->dev_fields[k]];
+        const SlotCol& sc = s.col[(size_t)x->dev_fields[k]];
         if (f.var()) {
             // (values_bytes = the bytes staged into this chunk: the offsets were built here, so the partitioner need not read them back)
-            in[k] = dfd_column{f.kind, 0, s.d_in[i], s.d_in_off[i], s.has_valid[i] ? (uint8_t*)s.d_in_valid[i] : nullptr, 0, s.data_bytes[i]};
-            out[k] = dfd_column{f.kind, 0, s.d_out[i], s.d_out_off[i], s.has_valid[i] ? (uint8_t*)s.d_out_valid[i] : nullptr, 0, (int64_t)s.out_cap[i]};
+            in[k] = dfd_column{f.kind, 0, sc.d_in, sc.d_in_off, sc.has_valid ? (uint8_t*)sc.d_in_valid : nullptr, 0, sc.data_bytes};
+            out[k] = dfd_column{f.kind, 0, sc.d_out, sc.d_out_off, sc.has_valid ? (uint8_t*)sc.d_out_valid : nullptr, 0, (int64_t)sc.out_cap};
         } else {
-            in[k] = dfd_column{f.kind, f.width, s.d_in[i], nullptr, s.has_valid[i] ? (uint8_t*)s.d_in_valid[i] : nullptr, 0, 0};
-            out[k] = dfd_column{f.kind, f.width, s.d_out[i], nullptr, s.has_valid[i] ? (uint8_t*)s.d_out_valid[i] : nullptr, 0, 0};
+            in[k] = dfd_column{f.kind, f.width, sc.d_in, nullptr, sc.has_valid ? (uint8_t*)sc.d_in_valid : nullptr, 0, 0};
+            out[k] = dfd_column{f.kind, f.width, sc.d_out, nullptr, sc.has_valid ? (uint8_t*)sc.d_out_valid : nullptr, 0, 0};
         }
         if (f.kind == DFD_COL_BOOL)
-            XCUDA(x, cudaMemsetAsync(s.d_out[i], 0, PinnedPool::bitmap_bytes(s.rows), c->stream), "memset");
-        if (s.has_valid[i]) XCUDA(x, cudaMemsetAsync(s.d_out_valid[i], 0, PinnedPool::bitmap_bytes(s.rows), c->stream), "memset");
+            XCUDA(x, cudaMemsetAsync(sc.d_out, 0, PinnedPool::bitmap_bytes(s.rows), c->stream), "memset");
+        if (sc.has_valid) XCUDA(x, cudaMemsetAsync(sc.d_out_valid, 0, PinnedPool::bitmap_bytes(s.rows), c->stream), "memset");
     }
     for (size_t i = 0; i < C; ++i)  // dictionary keys of this chunk (caller holds the context lock: set the fields directly)
         if (x->fields[i].dict && x->key_of_field[i] >= 0) {
             x->part->key_modes[(size_t)x->key_of_field[i]] = dfd::KEY_HASH_DICTIONARY;
-            x->part->key_dicts[(size_t)x->key_of_field[i]] = dfd_partitioner::KeyDict{s.dict_hashes[i], s.dict_valid[i], x->fields[i].dict_index_unsigned};
+            x->part->key_dicts[(size_t)x->key_of_field[i]] = dfd_partitioner::KeyDict{s.col[i].dict_hashes, s.col[i].dict_valid, x->fields[i].dict_index_unsigned};
         }
     int rc = partition_device_locked(x->part, in.data(), (int)D, s.rows, out.data(), c->stream, /*var_bytes_known=*/true);
     if (rc) return fail(x, rc, dfd_last_error());
@@ -730,24 +745,24 @@ int flush_current(dfd_repartition_exec* x) {
     for (size_t i = 0; i < x->n_visible; ++i) {
         const FieldInfo& f = x->fields[i];
         if (!f.list) continue;
-        const int64_t ne = s.data_bytes[(size_t)f.h_len] / 4;
+        const int64_t ne = s.col[(size_t)f.h_len].data_bytes / 4;
         auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
         const size_t o_off = 0, o_bits = al((size_t)(ne + 1) * 4 + 16), o_sums = o_bits + al((size_t)(ne + 63) / 64 * 8 + 16);
         const size_t total = o_sums + al((size_t)(ne / 2048 + 4) * 8);
-        int rc2 = s.list_tmp[i].ensure(total, c->device);
+        int rc2 = s.col[i].list_tmp.ensure(total, c->device);
         if (rc2) return fail(x, rc2, dfd_last_error());
-        char* lt = (char*)s.list_tmp[i].ptr;
+        char* lt = (char*)s.col[i].list_tmp.ptr;
         if (f.child_width > 0) {  // primitive child: no child offsets; the gathered lengths themselves are not needed on the host
             d2h_src[(size_t)f.h_len] = lt + o_off;
             d2h_nb[(size_t)f.h_len] = 0;
         } else {
-            if ((rc2 = launch_lengths_to_offsets(s.d_out[(size_t)f.h_len], 4, ne, (unsigned long long*)(lt + o_sums), lt + o_off, c->stream)))
+            if ((rc2 = launch_lengths_to_offsets(s.col[(size_t)f.h_len].d_out, 4, ne, (unsigned long long*)(lt + o_sums), lt + o_off, c->stream)))
                 return fail(x, rc2, dfd_last_error());
             d2h_src[(size_t)f.h_len] = lt + o_off;
             d2h_nb[(size_t)f.h_len] = (size_t)(ne + 1) * 4;
         }
         if (f.h_valid >= 0) {
-            if ((rc2 = launch_bytes_to_bits((const uint8_t*)s.d_out[(size_t)f.h_valid], ne, lt + o_bits, c->stream))) return fail(x, rc2, dfd_last_error());
+            if ((rc2 = launch_bytes_to_bits((const uint8_t*)s.col[(size_t)f.h_valid].d_out, ne, lt + o_bits, c->stream))) return fail(x, rc2, dfd_last_error());
             d2h_src[(size_t)f.h_valid] = lt + o_bits;
             d2h_nb[(size_t)f.h_valid] = (size_t)((ne + 31) / 32 * 4);
         }
@@ -761,10 +776,11 @@ int flush_current(dfd_repartition_exec* x) {
     for (size_t k = 0; k < D; ++k) {
         const size_t i = (size_t)x->dev_fields[k];
         const FieldInfo& f = x->fields[i];
+        const SlotCol& sc = s.col[i];
         size_t nb = f.kind == DFD_COL_BOOL ? (size_t)((s.rows + 7) / 8) : (size_t)s.rows * f.width;
-        const void* src = s.d_out[i];
+        const void* src = sc.d_out;
         if (f.var()) {
-            nb = (size_t)s.data_bytes[i];
+            nb = (size_t)sc.data_bytes;
             if (d2h_src[i]) { src = d2h_src[i]; nb = d2h_nb[i]; }  // list columns: scanned child offsets / re-packed child validity
             if (s.out->data_cap[i] < nb || !s.out->values[i]) {  // grow this pinned chunk's string buffer (never NULL, even for 0 bytes)
                 if (s.out->values[i]) cudaFreeHost(s.out->values[i]);
@@ -775,14 +791,14 @@ int flush_current(dfd_repartition_exec* x) {
                 s.out->data_cap[i] = want;
             }
             if (!f.hidden || f.role == 1) {  // (the per-row offsets of the hidden bytes / validity columns are not needed on the host)
-                XCUDA(x, cudaMemcpyAsync(s.out->offsets[i], s.d_out_off[i], (size_t)(s.rows + 1) * f.ow(), cudaMemcpyDeviceToHost, x->s_d2h), "D2H offsets");
+                XCUDA(x, cudaMemcpyAsync(s.out->offsets[i], sc.d_out_off, (size_t)(s.rows + 1) * f.ow(), cudaMemcpyDeviceToHost, x->s_d2h), "D2H offsets");
                 x->bytes_d2h += (size_t)(s.rows + 1) * f.ow();
             }
         }
         if (nb) XCUDA(x, cudaMemcpyAsync(s.out->values[i], src, nb, cudaMemcpyDeviceToHost, x->s_d2h), "D2H");
         x->bytes_d2h += nb;
-        if (s.has_valid[i]) {
-            XCUDA(x, cudaMemcpyAsync(s.out->validity[i], s.d_out_valid[i], (size_t)((s.rows + 7) / 8), cudaMemcpyDeviceToHost, x->s_d2h), "D2H");
+        if (sc.has_valid) {
+            XCUDA(x, cudaMemcpyAsync(s.out->validity[i], sc.d_out_valid, (size_t)((s.rows + 7) / 8), cudaMemcpyDeviceToHost, x->s_d2h), "D2H");
             x->bytes_d2h += (size_t)((s.rows + 7) / 8);
         }
     }
@@ -805,9 +821,11 @@ int open_next_slot(dfd_repartition_exec* x) {
         XCUDA(x, cudaStreamWaitEvent(x->s_h2d, s.e_k, 0), "wait k (h2d)");
     }
     s.rows = 0;
-    std::fill(s.has_valid.begin(), s.has_valid.end(), false);
-    std::fill(s.data_bytes.begin(), s.data_bytes.end(), 0);
-    std::fill(s.dict_id.begin(), s.dict_id.end(), DictId{});
+    for (SlotCol& sc : s.col) {
+        sc.has_valid = false;
+        sc.data_bytes = 0;
+        sc.dict_id = DictId{};
+    }
     x->cur_open = true;
     return DFD_OK;
 }
@@ -822,128 +840,48 @@ DictId dict_identity(const ArrowArray* d) {
     return DictId{d->n_buffers > 0 ? d->buffers[d->n_buffers - 1] : nullptr, d->offset, d->length};
 }
 
-bool same_dictionary(const FieldInfo& f, const ArrowArray* mine, const ArrowArray* theirs);
-int grow_var_bytes(dfd_repartition_exec* x, int64_t n, bool* fits);
-
-// Host-side preparation of rows [start, start + n) of `b` for the open chunk: where every variable-width device column's
-// offsets and bytes come from (views and lists are converted to offsets + bytes here, index arithmetic only), and whether
-// these rows can JOIN the chunk (`*fits`): same dictionaries, and string bytes within the offset width.  The chunk's
-// byte buffers grow here when the rows need more room.
-int prepare_rows(dfd_repartition_exec* x, const ArrowArray* b, int64_t start, int64_t n, bool* fits) {
-    Slot& s = x->slots[x->cur];
-    *fits = true;
-    for (size_t i = 0; i < x->n_visible; ++i) {
-        const FieldInfo& f = x->fields[i];
-        const ArrowArray* c = b->children[i];
-        const int64_t lo = c->offset + start;
-        if (validity_of(c) && !(f.flags & ARROW_FLAG_NULLABLE) && c->null_count > 0)
-            return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": nulls in a column the schema declares non-nullable");
-        if (f.list) {
-            // List<Utf8 / Binary> -> three hidden Binary columns: row -> its elements' int32 lengths, row -> its elements' bytes
-            // (one contiguous range of the child's data buffer), row -> one validity byte per element
-            if (c->n_children != 1 || !c->children[0]) return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": list array without a child");
-            const ArrowArray* v = c->children[0];
-            const int32_t* loff = (const int32_t*)c->buffers[1];
-            const int32_t cw = f.child_width;
-            const int32_t* coff = cw > 0 ? nullptr : (const int32_t*)v->buffers[1] + v->offset;
-            const uint8_t* cvalid = validity_of(v);
-            const int64_t e0 = loff[lo], e1 = loff[lo + n], ne = e1 - e0;
-            if (ne < 0) return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": list offsets are not monotonic");
-            if (ne * 4 > 0x7fffffffLL || ne * (int64_t)(cw > 0 ? cw : 1) > 0x7fffffffLL)
-                return fail(x, DFD_ERR_UNSUPPORTED, "column " + f.name + ": too many list elements in one chunk");
-            const size_t hl = (size_t)f.h_len, hb = (size_t)f.h_bytes;
-            std::vector<char>& ol = x->tmp_off[hl];
-            std::vector<char>& dl = x->tmp_bytes[hl];
-            std::vector<char>& ob = x->tmp_off[hb];
-            ol.resize((size_t)(n + 1) * 4);
-            ob.resize((size_t)(n + 1) * 4);
-            dl.resize((size_t)ne * 4 + 16);
-            int32_t* ov32 = nullptr;
-            char* dvb = nullptr;
-            if (f.h_valid >= 0) {
-                std::vector<char>& ov = x->tmp_off[(size_t)f.h_valid];
-                std::vector<char>& dv = x->tmp_bytes[(size_t)f.h_valid];
-                ov.resize((size_t)(n + 1) * 4);
-                dv.resize((size_t)ne + 16);
-                ov32 = (int32_t*)ov.data();
-                dvb = dv.data();
-            }
-            if (cw > 0) {
-                dfd::host::split_list_rows_fixed(loff, cw, cvalid, v->offset, lo, n, (int32_t*)ol.data(), (int32_t*)ob.data(), (int32_t*)dl.data(), ov32, dvb);
-                x->prep[hb] = VarPrep{ob.data(), 0, (const char*)v->buffers[1] + (size_t)(v->offset + e0) * (size_t)cw, ne * (int64_t)cw};
-            } else {
-                dfd::host::split_list_rows(loff, coff, cvalid, v->offset, lo, n, (int32_t*)ol.data(), (int32_t*)ob.data(), (int32_t*)dl.data(), ov32, dvb);
-                x->prep[hb] = VarPrep{ob.data(), 0, (const char*)v->buffers[2] + coff[e0], (int64_t)coff[e1] - coff[e0]};
-            }
-            x->prep[hl] = VarPrep{ol.data(), 0, dl.data(), ne * 4};
-            if (f.h_valid >= 0) x->prep[(size_t)f.h_valid] = VarPrep{(const char*)ov32, 0, dvb, ne};
-        } else if (f.var() && f.view) {
-            // Utf8View / BinaryView -> offsets + contiguous bytes (16-byte views: len | 12 inline bytes, or len | prefix |
-            // buffer index | offset into one of the variadic data buffers); from here on an ordinary Utf8 / Binary column
-            std::vector<char>& vo = x->tmp_off[i];
-            std::vector<char>& vb = x->tmp_bytes[i];
-            vo.resize((size_t)(n + 1) * 4);
-            int32_t* off32 = (int32_t*)vo.data();
-            const uint8_t* views = (const uint8_t*)c->buffers[1];
-            const int64_t total = dfd::host::view_offsets(views, validity_of(c), lo, n, off32);
-            if (total < 0) return fail(x, DFD_ERR_UNSUPPORTED, "column " + f.name + ": more than 2 GiB of view data in one chunk");
-            vb.resize((size_t)total + 16);
-            dfd::host::view_bytes(views, c->buffers + 2, lo, n, off32, vb.data());
-            x->prep[i] = VarPrep{vo.data(), 0, vb.data(), total};
-        } else if (f.var()) {
-            const size_t ow = f.ow();
-            const char* offs = (const char*)c->buffers[1];
-            int64_t first, last;
-            if (ow == 4) { first = ((const int32_t*)offs)[lo]; last = ((const int32_t*)offs)[lo + n]; }
-            else { first = ((const int64_t*)offs)[lo]; last = ((const int64_t*)offs)[lo + n]; }
-            if (last < first) return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": offsets are not monotonic");
-            x->prep[i] = VarPrep{offs + (size_t)lo * ow, first, (const char*)c->buffers[2] + first, last - first};
-        } else if (f.dict) {
-            if (!c->dictionary) return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": dictionary array without a dictionary");
-            // one dictionary per chunk (it travels by reference).  A batch whose dictionary is a different OBJECT with the same
-            // values (readers re-materialise the dictionary for every batch) joins the chunk and is served by the chunk's first one
-            const DictId id = dict_identity(c->dictionary);
-            if (s.rows > 0 && !(s.dict_id[i] == id)) {
-                const ArrowArray* mine = !s.held.empty() && s.held.front()->array.children[i] ? s.held.front()->array.children[i]->dictionary : nullptr;
-                if (!same_dictionary(f, mine, c->dictionary)) *fits = false;
-            }
-        }
-    }
-    if (!*fits) return DFD_OK;
-    return grow_var_bytes(x, n, fits);
-}
-
 // Does a dictionary with other buffers (`theirs`) hold the same values as the chunk's (`mine`)?  Both in host memory.
 bool same_dictionary(const FieldInfo& f, const ArrowArray* mine, const ArrowArray* theirs) {
-    const bool dvar = f.dict_kind == DFD_COL_UTF8 || f.dict_kind == DFD_COL_LARGE_UTF8 || f.dict_kind == DFD_COL_BINARY;
     const bool comparable = mine && f.dict_format[0] != 'v' && mine->length == theirs->length && mine->n_buffers == theirs->n_buffers &&
                             mine->length <= (1 << 16);  // (a linear comparison per batch: only worth it for small dictionaries — a batch's own)
-    return comparable && dfd::host::flat_arrays_equal(mine->length, dvar ? (f.dict_kind == DFD_COL_LARGE_UTF8 ? 8 : 4) : 0,
+    return comparable && dfd::host::flat_arrays_equal(mine->length, f.dict_var() ? (int)f.dict_ow() : 0,
                                                       f.dict_kind == DFD_COL_BOOL ? 0 : f.dict_width, mine->buffers, mine->offset, mine->null_count,
                                                       theirs->buffers, theirs->offset, theirs->null_count);
 }
 
-// The string bytes `x->prep` says rows [.., + n) add: cut the chunk early (`*fits` = false) when they would pass what 32-bit
-// offsets address, otherwise grow the chunk's byte buffers when they need more room.
+// the host waits for everything enqueued on the staging stream so far (read-backs of sizes / dictionaries of device input)
+int wait_staging(dfd_repartition_exec* x) {
+    {
+        std::lock_guard<std::mutex> lk(x->ctx->mu);
+        XCUDA(x, cudaSetDevice(x->ctx->device), "cudaSetDevice");
+        if (!x->e_sizes) XCUDA(x, cudaEventCreateWithFlags(&x->e_sizes, cudaEventDisableTiming), "cudaEventCreate");
+        XCUDA(x, cudaEventRecord(x->e_sizes, x->s_h2d), "record read-back");
+    }
+    XCUDA(x, cudaEventSynchronize(x->e_sizes), "read-back");
+    return DFD_OK;
+}
+
+// The string bytes the `prep` of the fields say rows [.., + n) add: cut the chunk early (`*fits` = false) when they would
+// pass what 32-bit offsets address, otherwise grow the chunk's byte buffers when they need more room.
 int grow_var_bytes(dfd_repartition_exec* x, int64_t n, bool* fits) {
     Slot& s = x->slots[x->cur];
     for (int fi : x->dev_fields) {
-        const size_t h = (size_t)fi;
-        const FieldInfo& f = x->fields[h];
+        const FieldInfo& f = x->fields[(size_t)fi];
+        SlotCol& sc = s.col[(size_t)fi];
         if (!f.var()) continue;
-        const int64_t need = s.data_bytes[h] + x->prep[h].nbytes;
+        const int64_t need = sc.data_bytes + x->tmp[(size_t)fi].prep.nbytes;
         if (f.ow() == 4 && need > 0x7fffffffLL) {
             if (s.rows > 0) { *fits = false; return DFD_OK; }
             return fail(x, DFD_ERR_UNSUPPORTED, "column " + f.name + ": more than 2 GiB of string data in one chunk (use a smaller chunk_rows or LargeUtf8)");
         }
-        if ((size_t)need <= s.in_cap[h]) continue;
+        if ((size_t)need <= sc.in_cap) continue;
         // grow the chunk's byte buffers, keeping what is already staged (the copy is ordered after the H2D appends on the same
         // stream; cudaFree waits for it).  Sized for a FULL chunk at the bytes per row seen so far, and at least doubled, so
         // that growth is rare and the following batches join the chunk instead of cutting it
         std::lock_guard<std::mutex> lk(x->ctx->mu);
         XCUDA(x, cudaSetDevice(x->ctx->device), "cudaSetDevice");
         size_t want = (size_t)need + (size_t)need / 4 + 256;
-        if (want < 2 * s.in_cap[h]) want = 2 * s.in_cap[h];
+        if (want < 2 * sc.in_cap) want = 2 * sc.in_cap;
         const double per_row = (double)need / (double)(s.rows + n);
         double full = per_row * (double)x->chunk_rows * 1.25;
         if (full > (double)(1ull << 30)) full = (double)(1ull << 30);
@@ -951,64 +889,257 @@ int grow_var_bytes(dfd_repartition_exec* x, int64_t n, bool* fits) {
         if (f.ow() == 4 && want > 0x7fffffffull + 256) want = 0x7fffffffull + 256;
         void* bigger = nullptr;
         XCUDA(x, cudaMalloc(&bigger, want), "cudaMalloc(string bytes)");
-        if (s.data_bytes[h] > 0) {
-            cudaError_t ce = cudaMemcpyAsync(bigger, s.d_in[h], (size_t)s.data_bytes[h], cudaMemcpyDeviceToDevice, x->s_h2d);
+        if (sc.data_bytes > 0) {
+            cudaError_t ce = cudaMemcpyAsync(bigger, sc.d_in, (size_t)sc.data_bytes, cudaMemcpyDeviceToDevice, x->s_h2d);
             if (ce != cudaSuccess) {
                 cudaFree(bigger);
                 return fail(x, DFD_ERR_CUDA, std::string("grow string bytes: ") + cudaGetErrorString(ce));
             }
         }
-        cudaFree(s.d_in[h]);
-        cudaFree(s.d_out[h]);
-        s.d_in[h] = bigger;
-        s.d_out[h] = nullptr;
-        s.in_cap[h] = want;
-        s.out_cap[h] = 0;
-        XCUDA(x, cudaMalloc(&s.d_out[h], want), "cudaMalloc(string bytes)");
-        s.out_cap[h] = want;
+        cudaFree(sc.d_in);
+        cudaFree(sc.d_out);
+        sc.d_in = bigger;
+        sc.d_out = nullptr;
+        sc.in_cap = want;
+        sc.out_cap = 0;
+        XCUDA(x, cudaMalloc(&sc.d_out, want), "cudaMalloc(string bytes)");
+        sc.out_cap = want;
     }
     return DFD_OK;
 }
 
-// copy rows [start, start + n) of `b` (prepared by prepare_rows) to the end of the open chunk.  Fixed-width values and
-// string bytes go to the device straight from the batch; bitmaps (validity, boolean values) and string offsets are
-// concatenated on the host — bit-granular, offsets re-based onto the chunk's byte buffer — and follow when the chunk is
+struct ViewTmp {  // byte offsets of the parts of a view field's device scratch, for n rows and `nbuf` variadic buffers
+    size_t lens, off, sums, ptrs, total;
+    ViewTmp(int64_t n, int64_t nbuf) {
+        auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
+        lens = 0;
+        off = al((size_t)n * 4 + 16);
+        sums = off + al((size_t)(n + 1) * 4 + 16);
+        ptrs = sums + al((size_t)(n / 2048 + 4) * 8);
+        total = ptrs + al((size_t)(nbuf > 0 ? nbuf : 1) * 8);
+    }
+};
+
+// Host input: what rows [start, start + n) of the visible variable-width fields span, read from the batch.  View fields are
+// converted to offsets + contiguous bytes here (16-byte views: len | 12 inline bytes, or len | prefix | buffer index |
+// offset into one of the variadic data buffers); from then on they are ordinary Utf8 / Binary columns.
+void measure_host(dfd_repartition_exec* x, const ArrowArray* b, int64_t start, int64_t n) {
+    for (size_t i = 0; i < x->n_visible; ++i) {
+        const FieldInfo& f = x->fields[i];
+        const ArrowArray* c = b->children[i];
+        const int64_t lo = c->offset + start;
+        FieldTmp& t = x->tmp[i];
+        if (f.list) {
+            const int32_t* loff = (const int32_t*)c->buffers[1];
+            t.span = Span{loff[lo], loff[lo + n]};
+            if (f.child_width == 0 && t.span.last >= t.span.first) {  // (decreasing list offsets are refused without reading the child's)
+                const ArrowArray* v = c->children[0];
+                const int32_t* coff = (const int32_t*)v->buffers[1] + v->offset;
+                t.span.child_first = coff[t.span.first];
+                t.span.child_last = coff[t.span.last];
+            }
+        } else if (f.view) {
+            t.off.resize((size_t)(n + 1) * 4);
+            int32_t* off32 = (int32_t*)t.off.data();
+            const uint8_t* views = (const uint8_t*)c->buffers[1];
+            const int64_t total = dfd::host::view_offsets(views, validity_of(c), lo, n, off32);  // (-1: past 32-bit offsets)
+            if (total >= 0) {
+                t.bytes.resize((size_t)total + 16);
+                dfd::host::view_bytes(views, c->buffers + 2, lo, n, off32, t.bytes.data());
+            }
+            t.span = Span{0, total};
+        } else if (f.var()) {
+            const void* offs = c->buffers[1];
+            if (f.ow() == 4) t.span = Span{((const int32_t*)offs)[lo], ((const int32_t*)offs)[lo + n]};
+            else t.span = Span{((const int64_t*)offs)[lo], ((const int64_t*)offs)[lo + n]};
+        }
+    }
+}
+
+// Device input: the same spans, computed by k_stage_sizes for all such fields at once and read back (one small D2H and one
+// wait; never for schemas without variable-width fields).  View fields also get their lengths' scan in the device scratch.
+int measure_device(dfd_repartition_exec* x, const ArrowArray* b, int64_t start, int64_t n) {
+    std::vector<StageSize> jobs;
+    std::vector<size_t> job_field;
+    for (size_t i = 0; i < x->n_visible; ++i) {
+        const FieldInfo& f = x->fields[i];
+        const ArrowArray* c = b->children[i];
+        StageSize j;
+        j.lo = c->offset + start;
+        j.n = n;
+        j.off = c->buffers[1];
+        if (f.list) {
+            const ArrowArray* v = c->children[0];
+            j.op = STAGE_SIZE_LIST;
+            j.off2 = f.child_width > 0 ? nullptr : (const int32_t*)v->buffers[1] + v->offset;
+        } else if (f.view) {
+            j.op = STAGE_SIZE_VIEW;  // (j.lens: set once the field's scratch is sized, below)
+            j.valid = validity_of(c);
+        } else if (f.var()) {
+            j.op = STAGE_SIZE_RANGE;
+            j.ow = (int32_t)f.ow();
+        } else {
+            continue;
+        }
+        jobs.push_back(j);
+        job_field.push_back(i);
+    }
+    if (jobs.empty()) return DFD_OK;
+    const size_t nb = jobs.size() * 4 * sizeof(int64_t);
+    {
+        std::lock_guard<std::mutex> lk(x->ctx->mu);
+        XCUDA(x, cudaSetDevice(x->ctx->device), "cudaSetDevice");
+        if (int rc = x->d_sizes.ensure(nb, x->ctx->device)) return fail(x, rc, dfd_last_error());
+        if (!x->h_sizes) XCUDA(x, cudaHostAlloc((void**)&x->h_sizes, x->fields.size() * 4 * sizeof(int64_t), cudaHostAllocPortable), "cudaHostAlloc(sizes)");
+        for (size_t k = 0; k < jobs.size(); ++k) {
+            jobs[k].out = (int64_t*)x->d_sizes.ptr + 4 * k;
+            if (jobs[k].op != STAGE_SIZE_VIEW) continue;
+            const ViewTmp vt(n, b->children[job_field[k]]->n_buffers - 3);
+            if (int rc = x->tmp[job_field[k]].view_dev.ensure(vt.total, x->ctx->device)) return fail(x, rc, dfd_last_error());
+            jobs[k].lens = (int32_t*)((char*)x->tmp[job_field[k]].view_dev.ptr + vt.lens);
+        }
+        XCUDA(x, cudaMemsetAsync(x->d_sizes.ptr, 0, nb, x->s_h2d), "memset sizes");
+        int rc = launch_stage_sizes(jobs.data(), (int)jobs.size(), x->s_h2d);
+        for (size_t k = 0; k < jobs.size() && !rc; ++k) {  // views: offsets = exclusive scan of the lengths
+            if (jobs[k].op != STAGE_SIZE_VIEW) continue;
+            const ViewTmp vt(n, b->children[job_field[k]]->n_buffers - 3);
+            char* t = (char*)x->tmp[job_field[k]].view_dev.ptr;
+            rc = launch_lengths_to_offsets(t + vt.lens, 4, n, (unsigned long long*)(t + vt.sums), t + vt.off, x->s_h2d);
+        }
+        if (rc) return fail(x, rc, dfd_last_error());
+        XCUDA(x, cudaMemcpyAsync(x->h_sizes, x->d_sizes.ptr, nb, cudaMemcpyDeviceToHost, x->s_h2d), "D2H sizes");
+    }
+    if (int rc = wait_staging(x)) return rc;
+    for (size_t k = 0; k < jobs.size(); ++k) {
+        const int64_t* r = x->h_sizes + 4 * k;
+        x->tmp[job_field[k]].span = jobs[k].op == STAGE_SIZE_VIEW ? Span{0, r[0]} : Span{r[0], r[1], r[2], r[3]};
+    }
+    return DFD_OK;
+}
+
+// Can rows [start, start + n) of `b` join the open chunk (`*fits`), and what do they add?  One pass over the columns checks
+// what the schema promises and cuts the chunk at another dictionary; the spans of the variable-width fields are measured
+// where the batch lives and checked here; then the chunk's byte buffers grow, or the chunk is cut when the rows' string
+// bytes would pass what 32-bit offsets address.
+int prepare_rows(dfd_repartition_exec* x, const ArrowArray* b, const HeldInput& dicts, int64_t start, int64_t n, bool* fits) {
+    Slot& s = x->slots[x->cur];
+    *fits = true;
+    for (size_t i = 0; i < x->n_visible; ++i) {
+        const FieldInfo& f = x->fields[i];
+        const ArrowArray* c = b->children[i];
+        if (validity_of(c) && !(f.flags & ARROW_FLAG_NULLABLE) && c->null_count > 0)
+            return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": nulls in a column the schema declares non-nullable");
+        if (f.list && (c->n_children != 1 || !c->children[0]))
+            return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": list array without a child");
+        if (!f.dict) continue;
+        if (!c->dictionary) return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": dictionary array without a dictionary");
+        // one dictionary per chunk (it travels by reference).  A batch whose dictionary is a different OBJECT with the same
+        // values (readers re-materialise the dictionary for every batch) joins the chunk and is served by the chunk's first
+        // one.  Identities are those of the batch's own dictionary; values are compared in host memory (`dicts`)
+        const DictId id = dict_identity(c->dictionary);
+        if (s.rows == 0) {
+            s.col[i].dict_id = id;
+        } else if (!(s.col[i].dict_id == id)) {
+            const ArrowArray* mine = !s.dict_held.empty() ? s.dict_held.front()->array.children[i]->dictionary : nullptr;
+            if (!same_dictionary(f, mine, dicts->array.children[i]->dictionary)) *fits = false;
+        }
+    }
+    if (!*fits) return DFD_OK;
+    if (x->input_mode == INPUT_DEVICE) {
+        if (int rc = measure_device(x, b, start, n)) return rc;
+    } else {
+        measure_host(x, b, start, n);
+    }
+    for (size_t i = 0; i < x->n_visible; ++i) {
+        const FieldInfo& f = x->fields[i];
+        const Span& sp = x->tmp[i].span;
+        if (f.list) {
+            const int64_t ne = sp.last - sp.first, cw = f.child_width;
+            if (ne < 0 || (cw == 0 && sp.child_last < sp.child_first))
+                return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": list offsets are not monotonic");
+            if (ne * 4 > 0x7fffffffLL || ne * (cw > 0 ? cw : 1) > 0x7fffffffLL)
+                return fail(x, DFD_ERR_UNSUPPORTED, "column " + f.name + ": too many list elements in one chunk");
+            x->tmp[(size_t)f.h_len].prep = VarPrep{0, ne * 4};
+            x->tmp[(size_t)f.h_bytes].prep = VarPrep{0, cw > 0 ? ne * cw : sp.child_last - sp.child_first};
+            if (f.h_valid >= 0) x->tmp[(size_t)f.h_valid].prep = VarPrep{0, ne};
+        } else if (f.view) {
+            if (sp.last < 0 || sp.last > 0x7fffffffLL) return fail(x, DFD_ERR_UNSUPPORTED, "column " + f.name + ": more than 2 GiB of view data in one chunk");
+            x->tmp[i].prep = VarPrep{0, sp.last};
+        } else if (f.var()) {
+            if (sp.last < sp.first) return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": offsets are not monotonic");
+            x->tmp[i].prep = VarPrep{sp.first, sp.last - sp.first};
+        }
+    }
+    return grow_var_bytes(x, n, fits);
+}
+
+size_t dict_hash_bytes(int64_t length) { return (size_t)(length + 1) * 8; }
+
+// bytes of the values [0, offset + length) of dictionary `d`, which is in host memory
+size_t dict_value_bytes(const FieldInfo& f, const ArrowArray* d) {
+    const int64_t dn = d->offset + d->length;
+    if (f.dict_kind == DFD_COL_BOOL) return (size_t)((dn + 7) / 8);
+    if (!f.dict_var()) return (size_t)dn * f.dict_width;
+    return (size_t)(f.dict_ow() == 8 ? ((const int64_t*)d->buffers[1])[dn] : ((const int32_t*)d->buffers[1])[dn]);
+}
+
+// Dictionary KEY field i: hash its values once per chunk on the device (DataFusion hash_dictionary); the chunk's rows pick
+// dict_hashes[index].  `values` are in device memory; the hashes go to the front of the slot's dict_buf (host input copies
+// the values behind them).  Caller holds the context lock.
+int hash_dictionary(dfd_repartition_exec* x, size_t i, dfd_column values, int64_t length) {
+    const FieldInfo& f = x->fields[i];
+    SlotCol& sc = x->slots[x->cur].col[i];
+    // the validity handed to the partitioner is indexed by dictionary index (0-based): it must start at the values' first bit
+    if (values.validity && values.offset != 0)
+        return fail(x, DFD_ERR_UNSUPPORTED, "column " + f.name + ": sliced dictionary values with nulls are not supported yet");
+    values.kind = f.dict_hash_kind();  // (interval values hash field by field, as interval keys do)
+    int rc = sc.dict_buf.ensure(dict_hash_bytes(length), x->ctx->device);
+    if (!rc) rc = hash_columns_locked(x->ctx, &values, 1, length, nullptr, (uint64_t*)sc.dict_buf.ptr, x->s_h2d);
+    if (rc) return fail(x, rc, dfd_last_error());
+    sc.dict_hashes = (const uint64_t*)sc.dict_buf.ptr;
+    sc.dict_valid = values.validity;
+    return DFD_OK;
+}
+
+// Host input: copy rows [start, start + n) of `b` (admitted by prepare_rows) to the end of the open chunk.  Fixed-width
+// values and string bytes go to the device straight from the batch; bitmaps (validity, boolean values) and string offsets
+// are concatenated on the host — bit-granular, offsets re-based onto the chunk's byte buffer — and follow when the chunk is
 // flushed.  A column gets a validity bitmap from the first batch that has one (earlier rows count as valid).
-int stage_rows(dfd_repartition_exec* x, const ArrowArray* b, int64_t start, int64_t n) {
+int stage_rows_host(dfd_repartition_exec* x, const ArrowArray* b, const HeldInput&, int64_t start, int64_t n) {
     Slot& s = x->slots[x->cur];
     std::lock_guard<std::mutex> lk(x->ctx->mu);
     XCUDA(x, cudaSetDevice(x->ctx->device), "cudaSetDevice");
-    auto host_bitmap = [&](std::vector<uint8_t*>& v, size_t i) -> uint8_t* {
-        if (!v[i] && cudaHostAlloc((void**)&v[i], PinnedPool::bitmap_bytes(x->chunk_rows) + 8, cudaHostAllocPortable) != cudaSuccess) v[i] = nullptr;
-        return v[i];
+    auto host_bitmap = [&](uint8_t*& p) -> uint8_t* {
+        if (!p && cudaHostAlloc((void**)&p, PinnedPool::bitmap_bytes(x->chunk_rows) + 8, cudaHostAllocPortable) != cudaSuccess) p = nullptr;
+        return p;
     };
     auto stage_validity = [&](size_t i, const uint8_t* valid, int64_t lo) -> int {
-        if (!valid && !s.has_valid[i]) return DFD_OK;
-        uint8_t* hb = host_bitmap(s.h_valid, i);
+        SlotCol& sc = s.col[i];
+        if (!valid && !sc.has_valid) return DFD_OK;
+        uint8_t* hb = host_bitmap(sc.h_valid);
         if (!hb) return fail(x, DFD_ERR_OOM, "pinned host allocation failed");
-        if (!s.has_valid[i]) {
+        if (!sc.has_valid) {
             append_bits(hb, 0, nullptr, 0, s.rows);
-            s.has_valid[i] = true;
+            sc.has_valid = true;
         }
         append_bits(hb, s.rows, valid, lo, n);
         return DFD_OK;
     };
-    auto stage_var = [&](size_t h) -> int {
-        const VarPrep& p = x->prep[h];
-        const int64_t base = s.data_bytes[h];
+    auto stage_var = [&](size_t h, const void* off, const char* bytes) -> int {  // n + 1 source offsets (from prep.first), their bytes
+        SlotCol& sc = s.col[h];
+        const VarPrep& p = x->tmp[h].prep;
+        const int64_t delta = sc.data_bytes - p.first;
         if (x->fields[h].ow() == 4) {
-            int32_t* dst = (int32_t*)s.h_off[h] + s.rows;
-            const int32_t* src = (const int32_t*)p.off;
-            const int64_t delta = base - p.first;
+            int32_t* dst = (int32_t*)sc.h_off + s.rows;
+            const int32_t* src = (const int32_t*)off;
             for (int64_t r = 0; r <= n; ++r) dst[r] = (int32_t)(src[r] + delta);
         } else {
-            int64_t* dst = (int64_t*)s.h_off[h] + s.rows;
-            const int64_t* src = (const int64_t*)p.off;
-            const int64_t delta = base - p.first;
+            int64_t* dst = (int64_t*)sc.h_off + s.rows;
+            const int64_t* src = (const int64_t*)off;
             for (int64_t r = 0; r <= n; ++r) dst[r] = src[r] + delta;
         }
-        if (p.nbytes) XCUDA(x, cudaMemcpyAsync((char*)s.d_in[h] + base, p.bytes, (size_t)p.nbytes, cudaMemcpyHostToDevice, x->s_h2d), "H2D");
-        s.data_bytes[h] = base + p.nbytes;
+        if (p.nbytes) XCUDA(x, cudaMemcpyAsync((char*)sc.d_in + sc.data_bytes, bytes, (size_t)p.nbytes, cudaMemcpyHostToDevice, x->s_h2d), "H2D");
+        sc.data_bytes += p.nbytes;
         x->bytes_h2d += (size_t)p.nbytes;
         return DFD_OK;
     };
@@ -1019,58 +1150,208 @@ int stage_rows(dfd_repartition_exec* x, const ArrowArray* b, int64_t start, int6
         const int64_t lo = c->offset + start;
         const uint8_t* valid = (f.flags & ARROW_FLAG_NULLABLE) ? validity_of(c) : nullptr;
         if (f.list) {
-            if ((rc2 = stage_var((size_t)f.h_len)) || (rc2 = stage_var((size_t)f.h_bytes))) return rc2;
-            if (f.h_valid >= 0 && (rc2 = stage_var((size_t)f.h_valid))) return rc2;
+            // List<Utf8 / Binary / primitive> -> three hidden Binary columns: row -> its elements' int32 lengths, row -> its
+            // elements' bytes (one contiguous range of the child's data), row -> one validity byte per element
+            const ArrowArray* v = c->children[0];
+            const int32_t* loff = (const int32_t*)c->buffers[1];
+            const int32_t cw = f.child_width;
+            const int64_t e0 = x->tmp[i].span.first, ne = x->tmp[i].span.last - e0;
+            FieldTmp& tl = x->tmp[(size_t)f.h_len];
+            FieldTmp& tb = x->tmp[(size_t)f.h_bytes];
+            tl.off.resize((size_t)(n + 1) * 4);
+            tb.off.resize((size_t)(n + 1) * 4);
+            tl.bytes.resize((size_t)ne * 4 + 16);
+            int32_t* ov32 = nullptr;
+            char* dvb = nullptr;
+            if (f.h_valid >= 0) {
+                FieldTmp& tv = x->tmp[(size_t)f.h_valid];
+                tv.off.resize((size_t)(n + 1) * 4);
+                tv.bytes.resize((size_t)ne + 16);
+                ov32 = (int32_t*)tv.off.data();
+                dvb = tv.bytes.data();
+            }
+            const char* child_bytes;
+            if (cw > 0) {
+                dfd::host::split_list_rows_fixed(loff, cw, validity_of(v), v->offset, lo, n, (int32_t*)tl.off.data(), (int32_t*)tb.off.data(),
+                                                 (int32_t*)tl.bytes.data(), ov32, dvb);
+                child_bytes = (const char*)v->buffers[1] + (size_t)(v->offset + e0) * (size_t)cw;
+            } else {
+                dfd::host::split_list_rows(loff, (const int32_t*)v->buffers[1] + v->offset, validity_of(v), v->offset, lo, n, (int32_t*)tl.off.data(),
+                                           (int32_t*)tb.off.data(), (int32_t*)tl.bytes.data(), ov32, dvb);
+                child_bytes = (const char*)v->buffers[2] + x->tmp[i].span.child_first;
+            }
+            if ((rc2 = stage_var((size_t)f.h_len, tl.off.data(), tl.bytes.data())) || (rc2 = stage_var((size_t)f.h_bytes, tb.off.data(), child_bytes))) return rc2;
+            if (f.h_valid >= 0 && (rc2 = stage_var((size_t)f.h_valid, ov32, dvb))) return rc2;
             if ((rc2 = stage_validity((size_t)f.h_len, valid, lo))) return rc2;  // the list's own validity rides on the lengths column
             continue;
         }
-        if (f.dict && s.rows == 0) s.dict_id[i] = dict_identity(c->dictionary);
         if (f.dict && x->key_of_field[i] >= 0 && s.rows == 0) {
-            // dictionary KEY: hash the dictionary values once per chunk on the device (DataFusion hash_dictionary); rows pick dict_hashes[index]
+            // dictionary KEY: its values go to the device, behind the room for their hashes
             const ArrowArray* d = c->dictionary;
             const int64_t dn = d->offset + d->length;
-            const bool dvar = f.dict_kind == DFD_COL_UTF8 || f.dict_kind == DFD_COL_LARGE_UTF8 || f.dict_kind == DFD_COL_BINARY;
-            const size_t dow = f.dict_kind == DFD_COL_LARGE_UTF8 ? 8 : 4;
-            const bool dhv = d->null_count != 0 && d->n_buffers > 0 && d->buffers[0] != nullptr;
-            int64_t dbytes = 0;
-            if (dvar) dbytes = dow == 4 ? ((const int32_t*)d->buffers[1])[dn] : ((const int64_t*)d->buffers[1])[dn];
+            const uint8_t* dvalid = validity_of(d);
+            const size_t nb_off = f.dict_var() ? (size_t)(dn + 1) * f.dict_ow() : 0, vbytes = dict_value_bytes(f, d);
             auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
-            const size_t o_hash = 0, o_off = al((size_t)(d->length + 1) * 8), o_data = o_off + al(dvar ? (size_t)(dn + 1) * dow : 0);
-            const size_t vbytes = f.dict_kind == DFD_COL_BOOL ? (size_t)((dn + 7) / 8) : (dvar ? (size_t)dbytes : (size_t)dn * f.dict_width);
+            const size_t o_off = al(dict_hash_bytes(d->length)), o_data = o_off + al(nb_off);
             const size_t o_valid = o_data + al(vbytes + 16), total = o_valid + al((size_t)((dn + 7) / 8) + 16);
-            rc2 = s.dict_buf[i].ensure(total, x->ctx->device);
-            if (rc2) return fail(x, rc2, dfd_last_error());
-            char* db = (char*)s.dict_buf[i].ptr;
-            if (dvar) XCUDA(x, cudaMemcpyAsync(db + o_off, d->buffers[1], (size_t)(dn + 1) * dow, cudaMemcpyHostToDevice, x->s_h2d), "H2D dictionary offsets");
-            if (vbytes) XCUDA(x, cudaMemcpyAsync(db + o_data, d->buffers[dvar ? 2 : 1], vbytes, cudaMemcpyHostToDevice, x->s_h2d), "H2D dictionary values");
-            if (dhv) XCUDA(x, cudaMemcpyAsync(db + o_valid, d->buffers[0], (size_t)((dn + 7) / 8), cudaMemcpyHostToDevice, x->s_h2d), "H2D dictionary validity");
-            const int32_t dmode = interval_key_mode(f.dict_format);  // interval values hash field by field, as interval keys do
-            const int32_t hkind = dmode == DFD_KEY_HASH_INTERVAL_DAY_TIME ? COL_INTERVAL_DAY_TIME
-                                  : dmode == DFD_KEY_HASH_INTERVAL_MONTH_DAY_NANO ? COL_INTERVAL_MONTH_DAY_NANO : f.dict_kind;
-            dfd_column dc{hkind, f.dict_width, db + o_data, dvar ? (void*)(db + o_off) : nullptr, dhv ? (uint8_t*)(db + o_valid) : nullptr, d->offset,
-                          (int64_t)vbytes};
-            rc2 = hash_columns_locked(x->ctx, &dc, 1, d->length, nullptr, (uint64_t*)(db + o_hash), x->s_h2d);
-            if (rc2) return fail(x, rc2, dfd_last_error());
-            s.dict_hashes[i] = (const uint64_t*)(db + o_hash);
-            // the validity handed to the partitioner is indexed by dictionary index (0-based): re-base with the values' offset
-            s.dict_valid[i] = dhv ? (const uint8_t*)(db + o_valid) : nullptr;
-            if (dhv && d->offset != 0) return fail(x, DFD_ERR_UNSUPPORTED, "column " + f.name + ": sliced dictionary values with nulls are not supported yet");
-            x->bytes_h2d += vbytes + (dvar ? (size_t)(dn + 1) * dow : 0);
+            if ((rc2 = s.col[i].dict_buf.ensure(total, x->ctx->device))) return fail(x, rc2, dfd_last_error());
+            char* db = (char*)s.col[i].dict_buf.ptr;
+            if (nb_off) XCUDA(x, cudaMemcpyAsync(db + o_off, d->buffers[1], nb_off, cudaMemcpyHostToDevice, x->s_h2d), "H2D dictionary offsets");
+            if (vbytes) XCUDA(x, cudaMemcpyAsync(db + o_data, d->buffers[f.dict_var() ? 2 : 1], vbytes, cudaMemcpyHostToDevice, x->s_h2d), "H2D dictionary values");
+            if (dvalid) XCUDA(x, cudaMemcpyAsync(db + o_valid, dvalid, (size_t)((dn + 7) / 8), cudaMemcpyHostToDevice, x->s_h2d), "H2D dictionary validity");
+            x->bytes_h2d += vbytes + nb_off;
+            const dfd_column dc{f.dict_kind, f.dict_width, db + o_data, nb_off ? db + o_off : nullptr, dvalid ? (uint8_t*)(db + o_valid) : nullptr, d->offset,
+                                (int64_t)vbytes};
+            if ((rc2 = hash_dictionary(x, i, dc, d->length))) return rc2;
         }
-        if (f.var()) {
-            if ((rc2 = stage_var(i))) return rc2;
+        if (f.view) {
+            if ((rc2 = stage_var(i, x->tmp[i].off.data(), x->tmp[i].bytes.data()))) return rc2;
+        } else if (f.var()) {
+            if ((rc2 = stage_var(i, (const char*)c->buffers[1] + (size_t)lo * f.ow(), (const char*)c->buffers[2] + x->tmp[i].prep.first))) return rc2;
         } else if (f.kind == DFD_COL_FIXED) {
             const char* src = (const char*)c->buffers[1] + (size_t)lo * f.width;
-            char* dst = (char*)s.d_in[i] + (size_t)s.rows * f.width;
+            char* dst = (char*)s.col[i].d_in + (size_t)s.rows * f.width;
             XCUDA(x, cudaMemcpyAsync(dst, src, (size_t)n * f.width, cudaMemcpyHostToDevice, x->s_h2d), "H2D");
             x->bytes_h2d += (size_t)n * f.width;
         } else {  // boolean values: one more bitmap
-            uint8_t* hb = host_bitmap(s.h_bool, i);
+            uint8_t* hb = host_bitmap(s.col[i].h_bool);
             if (!hb) return fail(x, DFD_ERR_OOM, "pinned host allocation failed");
             append_bits(hb, s.rows, (const uint8_t*)c->buffers[1], lo, n);
         }
         if ((rc2 = stage_validity(i, valid, lo))) return rc2;
     }
+    s.rows += n;
+    return DFD_OK;
+}
+
+// Device input: append rows [start, start + n) of the device batch `b` to the open chunk — every buffer of every column in
+// ONE k_stage_batch launch (plus a small H2D of the data buffer table of each view column).
+int stage_rows_device(dfd_repartition_exec* x, const ArrowArray* b, const HeldInput& dicts, int64_t start, int64_t n) {
+    Slot& s = x->slots[x->cur];
+    std::lock_guard<std::mutex> lk(x->ctx->mu);
+    XCUDA(x, cudaSetDevice(x->ctx->device), "cudaSetDevice");
+    std::vector<StageJob> jobs;
+    auto validity = [&](size_t i, const uint8_t* valid, int64_t lo) {
+        SlotCol& sc = s.col[i];
+        if (!valid && !sc.has_valid) return;
+        StageJob j;
+        j.op = STAGE_BITS;
+        j.src = valid;
+        j.a = lo;
+        j.dst = sc.d_in_valid;
+        j.b = s.rows;
+        j.c = sc.has_valid ? s.rows : 0;  // the first batch with a validity bitmap: earlier rows of the chunk count as valid
+        j.n = n;
+        sc.has_valid = true;
+        jobs.push_back(j);
+    };
+    auto offsets = [&](size_t h, const void* src, int ow_in, int64_t scale) {
+        StageJob j;
+        j.op = STAGE_OFFSETS;
+        j.src = src;
+        j.ow_in = ow_in;
+        j.ow_out = (int32_t)x->fields[h].ow();
+        j.dst = (char*)s.col[h].d_in_off + (size_t)s.rows * x->fields[h].ow();
+        j.n = n;
+        j.base = s.col[h].data_bytes;
+        j.scale = scale;
+        return j;
+    };
+    auto bytes = [&](size_t h, StageJob j) {  // (after the column's offsets job, which takes the old byte count as its base)
+        j.dst = (char*)s.col[h].d_in + s.col[h].data_bytes;
+        jobs.push_back(j);
+        s.col[h].data_bytes += x->tmp[h].prep.nbytes;
+    };
+    for (size_t i = 0; i < x->n_visible; ++i) {
+        const FieldInfo& f = x->fields[i];
+        const ArrowArray* c = b->children[i];
+        const int64_t lo = c->offset + start;
+        const uint8_t* valid = (f.flags & ARROW_FLAG_NULLABLE) ? validity_of(c) : nullptr;
+        if (f.list) {
+            const ArrowArray* v = c->children[0];
+            const size_t hl = (size_t)f.h_len, hb = (size_t)f.h_bytes;
+            const int32_t* loff = (const int32_t*)c->buffers[1] + lo;
+            const int32_t* coff = f.child_width > 0 ? nullptr : (const int32_t*)v->buffers[1] + v->offset;
+            const int64_t e0 = x->tmp[i].span.first, ne = x->tmp[i].span.last - e0, cw = f.child_width;
+            jobs.push_back(offsets(hl, loff, 4, 4));
+            StageJob len;
+            if (cw > 0) { len.op = STAGE_FILL32; len.base = cw; }
+            else { len.op = STAGE_DIFF32; len.src = coff + e0; }
+            len.n = ne;
+            bytes(hl, len);
+            if (cw > 0) {
+                jobs.push_back(offsets(hb, loff, 4, cw));
+            } else {
+                StageJob lo_ = offsets(hb, loff, 4, 1);
+                lo_.op = STAGE_LIST_OFFSETS;
+                lo_.src2 = coff;
+                jobs.push_back(lo_);
+            }
+            StageJob cp;
+            cp.src = cw > 0 ? (const char*)v->buffers[1] + (size_t)(v->offset + e0) * (size_t)cw : (const char*)v->buffers[2] + x->tmp[i].span.child_first;
+            cp.n = x->tmp[hb].prep.nbytes;
+            bytes(hb, cp);
+            if (f.h_valid >= 0) {
+                const size_t hv = (size_t)f.h_valid;
+                jobs.push_back(offsets(hv, loff, 4, 1));
+                StageJob vb;
+                vb.op = STAGE_BIT_BYTES;
+                vb.src = validity_of(v);
+                vb.a = v->offset + e0;
+                vb.n = ne;
+                bytes(hv, vb);
+            }
+            validity(hl, valid, lo);  // the list's own validity rides on the lengths column
+            continue;
+        }
+        if (f.dict && x->key_of_field[i] >= 0 && s.rows == 0) {
+            // dictionary KEY: hash the device-resident values in place (the first batch of the chunk stays held until its D2H
+            // is done); the host copy gives the byte count of string values
+            const ArrowArray* d = c->dictionary;
+            const dfd_column dc{f.dict_kind, f.dict_width, (void*)d->buffers[f.dict_var() ? 2 : 1], f.dict_var() ? (void*)d->buffers[1] : nullptr,
+                                (uint8_t*)validity_of(d), d->offset, (int64_t)dict_value_bytes(f, dicts->array.children[i]->dictionary)};
+            if (int rc = hash_dictionary(x, i, dc, d->length)) return rc;
+        }
+        if (f.view) {
+            // Utf8View / BinaryView: lengths and their scan came with the sizes; the data buffer table goes to the device
+            const int64_t nbuf = c->n_buffers - 3;  // (validity, views, data buffers..., variadic sizes: the sizes are not read)
+            const ViewTmp vt(n, nbuf);
+            char* t = (char*)x->tmp[i].view_dev.ptr;
+            if (nbuf > 0)
+                XCUDA(x, cudaMemcpyAsync(t + vt.ptrs, c->buffers + 2, (size_t)nbuf * sizeof(void*), cudaMemcpyHostToDevice, x->s_h2d), "H2D view buffer table");
+            jobs.push_back(offsets(i, t + vt.off, 4, 1));
+            StageJob vb;
+            vb.op = STAGE_VIEW_BYTES;
+            vb.src = (const uint8_t*)c->buffers[1] + (size_t)lo * 16;
+            vb.src2 = t + vt.ptrs;
+            vb.src3 = t + vt.off;
+            vb.n = n;
+            bytes(i, vb);
+        } else if (f.var()) {
+            jobs.push_back(offsets(i, (const char*)c->buffers[1] + (size_t)lo * f.ow(), (int)f.ow(), 1));
+            StageJob cp;
+            cp.src = (const char*)c->buffers[2] + x->tmp[i].prep.first;
+            cp.n = x->tmp[i].prep.nbytes;
+            bytes(i, cp);
+        } else if (f.kind == DFD_COL_FIXED) {
+            StageJob cp;
+            cp.src = (const char*)c->buffers[1] + (size_t)lo * f.width;
+            cp.dst = (char*)s.col[i].d_in + (size_t)s.rows * f.width;
+            cp.n = n * f.width;
+            jobs.push_back(cp);
+        } else {  // boolean values: one more bitmap
+            StageJob bv;
+            bv.op = STAGE_BITS;
+            bv.src = c->buffers[1];
+            bv.a = lo;
+            bv.dst = s.col[i].d_in;
+            bv.b = bv.c = s.rows;
+            bv.n = n;
+            jobs.push_back(bv);
+        }
+        validity(i, valid, lo);
+    }
+    if (int rc = launch_stage_batch(jobs.data(), (int)jobs.size(), x->s_h2d)) return fail(x, rc, dfd_last_error());
     s.rows += n;
     return DFD_OK;
 }
@@ -1086,20 +1367,6 @@ int emit_ready(dfd_repartition_exec* x) {
         int rc = emit_slot(x, s);
         if (rc) return rc;
     }
-    return DFD_OK;
-}
-
-// ---- device input (dfd_repartition_exec_push_device): the same chunks, assembled on the device by k_stage_* ---------------
-
-// the host waits for everything enqueued on the staging stream so far (read-backs of sizes / dictionaries)
-int wait_staging(dfd_repartition_exec* x) {
-    {
-        std::lock_guard<std::mutex> lk(x->ctx->mu);
-        XCUDA(x, cudaSetDevice(x->ctx->device), "cudaSetDevice");
-        if (!x->e_sizes) XCUDA(x, cudaEventCreateWithFlags(&x->e_sizes, cudaEventDisableTiming), "cudaEventCreate");
-        XCUDA(x, cudaEventRecord(x->e_sizes, x->s_h2d), "record read-back");
-    }
-    XCUDA(x, cudaEventSynchronize(x->e_sizes), "read-back");
     return DFD_OK;
 }
 
@@ -1146,8 +1413,8 @@ int host_dictionaries(dfd_repartition_exec* x, const ArrowArray* b, HeldInput* o
                 if (!d) continue;  // (prepare refuses a dictionary column without a dictionary)
                 const int64_t dn = d->offset + d->length;
                 const bool view = f.dict_format[0] == 'v';
-                const bool dvar = !view && (f.dict_kind == DFD_COL_UTF8 || f.dict_kind == DFD_COL_LARGE_UTF8 || f.dict_kind == DFD_COL_BINARY);
-                const size_t dow = f.dict_kind == DFD_COL_LARGE_UTF8 ? 8 : 4;
+                const bool dvar = !view && f.dict_var();
+                const size_t dow = f.dict_ow();
                 std::vector<const void*>& hb = h->bufs[i];
                 bool ok = true;
                 if (phase == 0) {
@@ -1194,261 +1461,6 @@ int host_dictionaries(dfd_repartition_exec* x, const ArrowArray* b, HeldInput* o
     return DFD_OK;
 }
 
-struct ViewTmp {  // byte offsets of the parts of a view field's device scratch, for n rows and `nbuf` variadic buffers
-    size_t lens, off, sums, ptrs, total;
-    ViewTmp(int64_t n, int64_t nbuf) {
-        auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
-        lens = 0;
-        off = al((size_t)n * 4 + 16);
-        sums = off + al((size_t)(n + 1) * 4 + 16);
-        ptrs = sums + al((size_t)(n / 2048 + 4) * 8);
-        total = ptrs + al((size_t)(nbuf > 0 ? nbuf : 1) * 8);
-    }
-};
-
-// Device counterpart of prepare_rows: the same checks and chunk cuts.  Variable-width columns need their byte counts on
-// the host (buffer growth, the 2 GiB cut of 32-bit offsets, values_bytes): k_stage_sizes computes them for all such
-// columns at once, and the host reads them back (one small D2H and one wait; never for fixed-width-only schemas).
-int prepare_rows_device(dfd_repartition_exec* x, const ArrowArray* b, const HeldInput& dicts, int64_t start, int64_t n, bool* fits) {
-    Slot& s = x->slots[x->cur];
-    *fits = true;
-    std::vector<StageSize> jobs;
-    std::vector<size_t> job_field;
-    for (size_t i = 0; i < x->n_visible; ++i) {
-        const FieldInfo& f = x->fields[i];
-        const ArrowArray* c = b->children[i];
-        const int64_t lo = c->offset + start;
-        if (validity_of(c) && !(f.flags & ARROW_FLAG_NULLABLE) && c->null_count > 0)
-            return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": nulls in a column the schema declares non-nullable");
-        StageSize j;
-        j.lo = lo;
-        j.n = n;
-        if (f.list) {
-            if (c->n_children != 1 || !c->children[0]) return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": list array without a child");
-            const ArrowArray* v = c->children[0];
-            j.op = STAGE_SIZE_LIST;
-            j.off = c->buffers[1];
-            j.off2 = f.child_width > 0 ? nullptr : (const int32_t*)v->buffers[1] + v->offset;
-        } else if (f.var() && f.view) {
-            j.op = STAGE_SIZE_VIEW;  // (j.lens: set once the field's scratch is sized, below)
-            j.off = c->buffers[1];
-            j.valid = validity_of(c);
-        } else if (f.var()) {
-            j.op = STAGE_SIZE_RANGE;
-            j.ow = (int32_t)f.ow();
-            j.off = c->buffers[1];
-        } else {
-            if (f.dict) {
-                if (!c->dictionary) return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": dictionary array without a dictionary");
-                const DictId id = dict_identity(c->dictionary);  // (identity of the DEVICE dictionary; values compared on the host copies)
-                if (s.rows > 0 && !(s.dict_id[i] == id)) {
-                    const ArrowArray* mine = !s.dict_held.empty() ? s.dict_held.front()->array.children[i]->dictionary : nullptr;
-                    if (!same_dictionary(f, mine, dicts->array.children[i]->dictionary)) *fits = false;
-                }
-            }
-            continue;
-        }
-        jobs.push_back(j);
-        job_field.push_back(i);
-    }
-    if (!*fits || jobs.empty()) return DFD_OK;
-    const size_t nb = jobs.size() * 4 * sizeof(int64_t);
-    {
-        std::lock_guard<std::mutex> lk(x->ctx->mu);
-        XCUDA(x, cudaSetDevice(x->ctx->device), "cudaSetDevice");
-        if (int rc = x->d_sizes.ensure(nb, x->ctx->device)) return fail(x, rc, dfd_last_error());
-        if (!x->h_sizes) XCUDA(x, cudaHostAlloc((void**)&x->h_sizes, x->fields.size() * 4 * sizeof(int64_t), cudaHostAllocPortable), "cudaHostAlloc(sizes)");
-        for (size_t k = 0; k < jobs.size(); ++k) {
-            jobs[k].out = (int64_t*)x->d_sizes.ptr + 4 * k;
-            if (jobs[k].op != STAGE_SIZE_VIEW) continue;
-            const ViewTmp vt(n, b->children[job_field[k]]->n_buffers - 3);
-            if (int rc = x->view_tmp[job_field[k]].ensure(vt.total, x->ctx->device)) return fail(x, rc, dfd_last_error());
-            jobs[k].lens = (int32_t*)((char*)x->view_tmp[job_field[k]].ptr + vt.lens);
-        }
-        XCUDA(x, cudaMemsetAsync(x->d_sizes.ptr, 0, nb, x->s_h2d), "memset sizes");
-        int rc = launch_stage_sizes(jobs.data(), (int)jobs.size(), x->s_h2d);
-        for (size_t k = 0; k < jobs.size() && !rc; ++k) {  // views: offsets = exclusive scan of the lengths
-            if (jobs[k].op != STAGE_SIZE_VIEW) continue;
-            const ViewTmp vt(n, b->children[job_field[k]]->n_buffers - 3);
-            char* t = (char*)x->view_tmp[job_field[k]].ptr;
-            rc = launch_lengths_to_offsets(t + vt.lens, 4, n, (unsigned long long*)(t + vt.sums), t + vt.off, x->s_h2d);
-        }
-        if (rc) return fail(x, rc, dfd_last_error());
-        XCUDA(x, cudaMemcpyAsync(x->h_sizes, x->d_sizes.ptr, nb, cudaMemcpyDeviceToHost, x->s_h2d), "D2H sizes");
-    }
-    if (int rc = wait_staging(x)) return rc;
-    for (size_t k = 0; k < jobs.size(); ++k) {
-        const size_t i = job_field[k];
-        const FieldInfo& f = x->fields[i];
-        const int64_t* r = x->h_sizes + 4 * k;
-        x->dsz[i].assign(r, r + 4);
-        if (f.list) {
-            const int64_t ne = r[1] - r[0], cw = f.child_width;
-            if (ne < 0 || (cw == 0 && r[3] < r[2])) return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": list offsets are not monotonic");
-            if (ne * 4 > 0x7fffffffLL || ne * (cw > 0 ? cw : 1) > 0x7fffffffLL)
-                return fail(x, DFD_ERR_UNSUPPORTED, "column " + f.name + ": too many list elements in one chunk");
-            x->prep[(size_t)f.h_len].nbytes = ne * 4;
-            x->prep[(size_t)f.h_bytes].nbytes = cw > 0 ? ne * cw : r[3] - r[2];
-            if (f.h_valid >= 0) x->prep[(size_t)f.h_valid].nbytes = ne;
-        } else if (f.view) {
-            if (r[0] > 0x7fffffffLL) return fail(x, DFD_ERR_UNSUPPORTED, "column " + f.name + ": more than 2 GiB of view data in one chunk");
-            x->prep[i].nbytes = r[0];
-        } else {
-            if (r[1] < r[0]) return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": offsets are not monotonic");
-            x->prep[i].first = r[0];
-            x->prep[i].nbytes = r[1] - r[0];
-        }
-    }
-    return grow_var_bytes(x, n, fits);
-}
-
-// Device counterpart of stage_rows: append rows [start, start + n) of the device batch `b` to the open chunk — every buffer
-// of every column in ONE k_stage_batch launch (plus a small H2D of the data buffer table of each view column).
-int stage_rows_device(dfd_repartition_exec* x, const ArrowArray* b, const HeldInput& dicts, int64_t start, int64_t n) {
-    Slot& s = x->slots[x->cur];
-    std::lock_guard<std::mutex> lk(x->ctx->mu);
-    XCUDA(x, cudaSetDevice(x->ctx->device), "cudaSetDevice");
-    std::vector<StageJob> jobs;
-    auto validity = [&](size_t i, const uint8_t* valid, int64_t lo) {
-        if (!valid && !s.has_valid[i]) return;
-        StageJob j;
-        j.op = STAGE_BITS;
-        j.src = valid;
-        j.a = lo;
-        j.dst = s.d_in_valid[i];
-        j.b = s.rows;
-        j.c = s.has_valid[i] ? s.rows : 0;  // the first batch with a validity bitmap: earlier rows of the chunk count as valid
-        j.n = n;
-        s.has_valid[i] = true;
-        jobs.push_back(j);
-    };
-    auto offsets = [&](size_t h, const void* src, int ow_in, int64_t scale) {
-        StageJob j;
-        j.op = STAGE_OFFSETS;
-        j.src = src;
-        j.ow_in = ow_in;
-        j.ow_out = (int32_t)x->fields[h].ow();
-        j.dst = (char*)s.d_in_off[h] + (size_t)s.rows * x->fields[h].ow();
-        j.n = n;
-        j.base = s.data_bytes[h];
-        j.scale = scale;
-        return j;
-    };
-    auto bytes = [&](size_t h, StageJob j) {  // (after the column's offsets job, which takes the old byte count as its base)
-        j.dst = (char*)s.d_in[h] + s.data_bytes[h];
-        jobs.push_back(j);
-        s.data_bytes[h] += x->prep[h].nbytes;
-    };
-    for (size_t i = 0; i < x->n_visible; ++i) {
-        const FieldInfo& f = x->fields[i];
-        const ArrowArray* c = b->children[i];
-        const int64_t lo = c->offset + start;
-        const uint8_t* valid = (f.flags & ARROW_FLAG_NULLABLE) ? validity_of(c) : nullptr;
-        if (f.list) {
-            const ArrowArray* v = c->children[0];
-            const size_t hl = (size_t)f.h_len, hb = (size_t)f.h_bytes;
-            const int32_t* loff = (const int32_t*)c->buffers[1] + lo;
-            const int32_t* coff = f.child_width > 0 ? nullptr : (const int32_t*)v->buffers[1] + v->offset;
-            const int64_t e0 = x->dsz[i][0], ne = x->dsz[i][1] - e0, cw = f.child_width;
-            jobs.push_back(offsets(hl, loff, 4, 4));
-            StageJob len;
-            if (cw > 0) { len.op = STAGE_FILL32; len.base = cw; }
-            else { len.op = STAGE_DIFF32; len.src = coff + e0; }
-            len.n = ne;
-            bytes(hl, len);
-            if (cw > 0) {
-                jobs.push_back(offsets(hb, loff, 4, cw));
-            } else {
-                StageJob lo_ = offsets(hb, loff, 4, 1);
-                lo_.op = STAGE_LIST_OFFSETS;
-                lo_.src2 = coff;
-                jobs.push_back(lo_);
-            }
-            StageJob cp;
-            cp.src = cw > 0 ? (const char*)v->buffers[1] + (size_t)(v->offset + e0) * (size_t)cw : (const char*)v->buffers[2] + x->dsz[i][2];
-            cp.n = x->prep[hb].nbytes;
-            bytes(hb, cp);
-            if (f.h_valid >= 0) {
-                const size_t hv = (size_t)f.h_valid;
-                jobs.push_back(offsets(hv, loff, 4, 1));
-                StageJob vb;
-                vb.op = STAGE_BIT_BYTES;
-                vb.src = validity_of(v);
-                vb.a = v->offset + e0;
-                vb.n = ne;
-                bytes(hv, vb);
-            }
-            validity(hl, valid, lo);  // the list's own validity rides on the lengths column
-            continue;
-        }
-        if (f.dict && s.rows == 0) s.dict_id[i] = dict_identity(c->dictionary);
-        if (f.dict && x->key_of_field[i] >= 0 && s.rows == 0) {
-            // dictionary KEY: hash the device-resident values in place once per chunk (DataFusion hash_dictionary)
-            const ArrowArray* d = c->dictionary;
-            const ArrowArray* hd = dicts->array.children[i]->dictionary;  // (host copy: the byte count of string values)
-            const int64_t dn = d->offset + d->length;
-            const bool dvar = f.dict_kind == DFD_COL_UTF8 || f.dict_kind == DFD_COL_LARGE_UTF8 || f.dict_kind == DFD_COL_BINARY;
-            const bool dhv = d->null_count != 0 && d->n_buffers > 0 && d->buffers[0] != nullptr;
-            int64_t dbytes = 0;
-            if (dvar) dbytes = f.dict_kind == DFD_COL_LARGE_UTF8 ? ((const int64_t*)hd->buffers[1])[dn] : ((const int32_t*)hd->buffers[1])[dn];
-            const size_t vbytes = f.dict_kind == DFD_COL_BOOL ? (size_t)((dn + 7) / 8) : (dvar ? (size_t)dbytes : (size_t)dn * f.dict_width);
-            int rc = s.dict_buf[i].ensure((size_t)(d->length + 1) * 8, x->ctx->device);
-            if (rc) return fail(x, rc, dfd_last_error());
-            const int32_t dmode = interval_key_mode(f.dict_format);
-            const int32_t hkind = dmode == DFD_KEY_HASH_INTERVAL_DAY_TIME ? COL_INTERVAL_DAY_TIME
-                                  : dmode == DFD_KEY_HASH_INTERVAL_MONTH_DAY_NANO ? COL_INTERVAL_MONTH_DAY_NANO : f.dict_kind;
-            dfd_column dc{hkind, f.dict_width, (void*)d->buffers[dvar ? 2 : 1], dvar ? (void*)d->buffers[1] : nullptr, dhv ? (uint8_t*)d->buffers[0] : nullptr,
-                          d->offset, (int64_t)vbytes};
-            rc = hash_columns_locked(x->ctx, &dc, 1, d->length, nullptr, (uint64_t*)s.dict_buf[i].ptr, x->s_h2d);
-            if (rc) return fail(x, rc, dfd_last_error());
-            s.dict_hashes[i] = (const uint64_t*)s.dict_buf[i].ptr;
-            s.dict_valid[i] = dhv ? (const uint8_t*)d->buffers[0] : nullptr;  // (the first batch of the chunk stays held until its D2H is done)
-            if (dhv && d->offset != 0) return fail(x, DFD_ERR_UNSUPPORTED, "column " + f.name + ": sliced dictionary values with nulls are not supported yet");
-        }
-        if (f.var() && f.view) {
-            // Utf8View / BinaryView: lengths and their scan came with the sizes; the data buffer table goes to the device
-            const int64_t nbuf = c->n_buffers - 3;  // (validity, views, data buffers..., variadic sizes: the sizes are not read)
-            const ViewTmp vt(n, nbuf);
-            char* t = (char*)x->view_tmp[i].ptr;
-            if (nbuf > 0)
-                XCUDA(x, cudaMemcpyAsync(t + vt.ptrs, c->buffers + 2, (size_t)nbuf * sizeof(void*), cudaMemcpyHostToDevice, x->s_h2d), "H2D view buffer table");
-            jobs.push_back(offsets(i, t + vt.off, 4, 1));
-            StageJob vb;
-            vb.op = STAGE_VIEW_BYTES;
-            vb.src = (const uint8_t*)c->buffers[1] + (size_t)lo * 16;
-            vb.src2 = t + vt.ptrs;
-            vb.src3 = t + vt.off;
-            vb.n = n;
-            bytes(i, vb);
-        } else if (f.var()) {
-            jobs.push_back(offsets(i, (const char*)c->buffers[1] + (size_t)lo * f.ow(), (int)f.ow(), 1));
-            StageJob cp;
-            cp.src = (const char*)c->buffers[2] + x->prep[i].first;
-            cp.n = x->prep[i].nbytes;
-            bytes(i, cp);
-        } else if (f.kind == DFD_COL_FIXED) {
-            StageJob cp;
-            cp.src = (const char*)c->buffers[1] + (size_t)lo * f.width;
-            cp.dst = (char*)s.d_in[i] + (size_t)s.rows * f.width;
-            cp.n = n * f.width;
-            jobs.push_back(cp);
-        } else {  // boolean values: one more bitmap
-            StageJob bv;
-            bv.op = STAGE_BITS;
-            bv.src = c->buffers[1];
-            bv.a = lo;
-            bv.dst = s.d_in[i];
-            bv.b = bv.c = s.rows;
-            bv.n = n;
-            jobs.push_back(bv);
-        }
-        validity(i, valid, lo);
-    }
-    if (int rc = launch_stage_batch(jobs.data(), (int)jobs.size(), x->s_h2d)) return fail(x, rc, dfd_last_error());
-    s.rows += n;
-    return DFD_OK;
-}
-
 // After an error or an abort of a device-input operator: wait for the device work that still reads the pushed batches,
 // then release them (the producer gets its memory back now, not when the operator is destroyed).
 void release_device_inputs(dfd_repartition_exec* x) {
@@ -1463,6 +1475,140 @@ void release_device_inputs(dfd_repartition_exec* x) {
         s.held.clear();
         s.dict_held.clear();
     }
+}
+
+// The device and pinned buffers of one pipeline slot: offsets and bitmaps for a full chunk now, string bytes on demand
+// (caller holds the context lock).  free_slot frees whatever it holds.
+cudaError_t alloc_slot(const dfd_repartition_exec* x, Slot& s) {
+    s.col.resize(x->fields.size());
+    const size_t bitmap = PinnedPool::bitmap_bytes(x->chunk_rows) + 8;
+    for (size_t i = 0; i < x->fields.size(); ++i) {
+        const FieldInfo& f = x->fields[i];
+        SlotCol& sc = s.col[i];
+        if (f.nodev()) continue;  // list placeholder: its rows live in the hidden columns
+        cudaError_t e;
+        if (f.var()) {
+            const size_t ob = (size_t)(x->chunk_rows + 16) * f.ow();
+            e = cudaMalloc(&sc.d_in_off, ob);
+            if (e == cudaSuccess) e = cudaHostAlloc((void**)&sc.h_off, ob, cudaHostAllocPortable);
+            if (e == cudaSuccess) e = cudaMalloc(&sc.d_out_off, ob);
+        } else {
+            const size_t vb = PinnedPool::value_bytes(f, x->chunk_rows) + 16 * (size_t)(f.width ? f.width : 1);
+            e = cudaMalloc(&sc.d_in, vb);
+            if (e == cudaSuccess) e = cudaMalloc(&sc.d_out, vb);
+        }
+        if (e == cudaSuccess && (f.flags & ARROW_FLAG_NULLABLE)) {
+            e = cudaMalloc(&sc.d_in_valid, bitmap);
+            if (e == cudaSuccess) e = cudaMalloc(&sc.d_out_valid, bitmap);
+        }
+        if (e != cudaSuccess) return e;
+    }
+    cudaError_t e = cudaHostAlloc((void**)&s.h_part_starts, sizeof(int64_t) * (x->N + 1), cudaHostAllocPortable);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s.e_h2d, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s.e_k, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s.e_d2h, cudaEventDisableTiming);
+    return e;
+}
+
+void free_slot(dfd_repartition_exec* x, Slot& s) {  // (caller holds the context lock, the streams are idle)
+    s.held.clear();
+    s.dict_held.clear();
+    if (s.out) { s.out->refs.store(1); s.out->pool = x->pool; chunk_unref(s.out); }
+    for (SlotCol& sc : s.col) {
+        for (void* p : {sc.d_in, sc.d_in_valid, sc.d_out, sc.d_out_valid, sc.d_in_off, sc.d_out_off, sc.dict_buf.ptr, sc.list_tmp.ptr}) cudaFree(p);
+        for (void* p : {(void*)sc.h_valid, (void*)sc.h_bool, (void*)sc.h_off})
+            if (p) cudaFreeHost(p);
+    }
+    if (s.h_part_starts) cudaFreeHost(s.h_part_starts);
+    if (s.e_h2d) cudaEventDestroy(s.e_h2d);
+    if (s.e_k) cudaEventDestroy(s.e_k);
+    if (s.e_d2h) cudaEventDestroy(s.e_d2h);
+}
+
+// A refused batch is released and the operator fails; a device-input operator also lets go of the batches it holds.
+int refuse(dfd_repartition_exec* x, ArrowArray* a, int code, const std::string& msg) {
+    if (a->release) a->release(a);
+    const int rc = fail(x, code, msg);
+    if (x->input_mode == INPUT_DEVICE) release_device_inputs(x);
+    return rc;
+}
+
+int refuse_after_finish(dfd_repartition_exec* x, ArrowArray* a) {  // (the operator's first outcome stands)
+    if (a->release) a->release(a);
+    return set_error(DFD_ERR_INVALID_ARGUMENT, "push after finish/error: %s", x->error.c_str());
+}
+
+// What push and push_device share after their own checks: the checks of the batch against the schema and the operator's
+// input kind, then the chunk loop.  Batches of every shape are APPENDED to the open chunk (bitmaps concatenated at bit
+// granularity, string offsets re-based); the chunk is cut early only when rows cannot join it: another dictionary, or
+// string bytes beyond what 32-bit offsets address.
+int push_rows(dfd_repartition_exec* x, ArrowArray* a, int mode, void* sync_event) {
+    if (a->n_children != (int64_t)x->n_visible)
+        return refuse(x, a, DFD_ERR_INVALID_ARGUMENT, "batch has " + std::to_string(a->n_children) + " columns, schema has " + std::to_string(x->n_visible));
+    const int64_t R = a->length;
+    x->rows_in += (uint64_t)R;
+    if (R == 0) {
+        if (a->release) a->release(a);
+        return DFD_OK;
+    }
+    if (x->input_mode != INPUT_UNSET && x->input_mode != mode)
+        return refuse(x, a, DFD_ERR_INVALID_ARGUMENT, mode == INPUT_HOST ? "host batch pushed to an operator that takes device batches (push_device)"
+                                                                        : "device batch pushed to an operator that takes host batches (push / run)");
+    for (int64_t i = 0; i < a->n_children; ++i)
+        if (a->children[i]->length < R || (a->offset != 0))
+            return refuse(x, a, DFD_ERR_INVALID_ARGUMENT, "record batch children shorter than the batch, or non-zero struct offset");
+    x->input_mode = mode;
+    if (sync_event) {  // the staging stream waits for the producer's work; the host does not
+        cudaError_t e;
+        {
+            std::lock_guard<std::mutex> lk(x->ctx->mu);
+            e = cudaSetDevice(x->ctx->device);
+            if (e == cudaSuccess) e = cudaStreamWaitEvent(x->s_h2d, *(cudaEvent_t*)sync_event, 0);
+        }
+        if (e != cudaSuccess) return refuse(x, a, DFD_ERR_CUDA, std::string("wait on the batch's sync_event: ") + cudaGetErrorString(e));
+    }
+    // ownership of the batch moves to a shared holder: every chunk that stages rows from it keeps it alive (host input: so
+    // does every output batch that references its dictionaries)
+    HeldInput holder = std::make_shared<SharedInput>(*a);
+    a->release = nullptr;
+    const ArrowArray* in = &holder->array;
+    auto bail = [&](int rc) {
+        if (mode == INPUT_DEVICE) release_device_inputs(x);
+        return rc;
+    };
+    int rc = DFD_OK;
+    HeldInput dicts;  // what the output batches' dictionaries reference: the batch itself, or host copies of a device batch's
+    for (const FieldInfo& f : x->fields)
+        if (f.dict) {
+            if (mode == INPUT_HOST) dicts = holder;
+            else if ((rc = host_dictionaries(x, in, &dicts))) return bail(rc);
+            break;
+        }
+    const auto stage_rows = mode == INPUT_HOST ? stage_rows_host : stage_rows_device;
+    int64_t done = 0;
+    while (done < R) {
+        if (!x->cur_open && (rc = open_next_slot(x))) return bail(rc);
+        Slot& s = x->slots[x->cur];
+        const int64_t room = x->chunk_rows - s.rows;
+        if (room == 0) {
+            if ((rc = flush_current(x))) return bail(rc);
+            continue;
+        }
+        const int64_t n = R - done < room ? R - done : room;
+        bool fits = true;
+        if ((rc = prepare_rows(x, in, dicts, done, n, &fits))) return bail(rc);
+        if (!fits) {
+            if ((rc = flush_current(x))) return bail(rc);
+            continue;  // (prepared again against an empty chunk, which always fits or grows)
+        }
+        if ((rc = stage_rows(x, in, dicts, done, n))) return bail(rc);
+        s.held.push_back(holder);
+        if (dicts) s.dict_held.push_back(dicts);
+        done += n;
+        if (s.rows == x->chunk_rows && (rc = flush_current(x))) return bail(rc);
+    }
+    if ((rc = emit_ready(x))) return bail(rc);
+    return DFD_OK;
 }
 
 }  // namespace
@@ -1480,7 +1626,7 @@ int dfd_arrow_format_layout(const char* format, int32_t* kind, int32_t* width) {
 
 // List<Utf8> / List<Binary> / List<fixed-width primitive> (int32 list offsets): the nested shapes the shuffle path moves
 // (payload only).  *child_width = 0 for string children, the value width for primitive ones (array_agg / median states).
-static bool list_child_ok(const ArrowSchema* c, int32_t* child_width = nullptr) {
+static bool list_child_ok(const ArrowSchema* c, int32_t* child_width) {
     if (!c->format || strcmp(c->format, "+l") != 0 || c->n_children != 1 || !c->children || !c->children[0]) return false;
     const ArrowSchema* v = c->children[0];
     if (!v->format || v->dictionary || v->n_children != 0) return false;
@@ -1488,26 +1634,39 @@ static bool list_child_ok(const ArrowSchema* c, int32_t* child_width = nullptr) 
     if (strcmp(v->format, "u") == 0 || strcmp(v->format, "z") == 0) w = 0;
     else if (parse_format(v->format, &k, &w) && k == DFD_COL_FIXED && v->format[0] != 'w') { /* ints, floats, decimals, dates, times */ }
     else return false;
-    if (child_width) *child_width = w;
+    *child_width = w;
     return true;
 }
 
-// One column of the record-batch schema: can the operator move it, and — if it is hash key `is_key` — hash it like DataFusion?
-static int check_column(const ArrowSchema* c, long long i, bool is_key) {
+// One column `i` of the record-batch schema: can the operator move it, and — if it is a hash key — hash it like DataFusion?
+// Fills `f` with what the operator keeps of it.
+static int describe_column(const ArrowSchema* c, long long i, bool is_key, FieldInfo* f) {
     const char* name = c->name ? c->name : "";
-    int32_t k, w;
-    if (list_child_ok(c)) {  // List<Utf8 / Binary>: payload only
+    f->name = name;
+    f->format = c->format ? c->format : "";
+    f->flags = c->flags;
+    if (list_child_ok(c, &f->child_width)) {  // List<Utf8 / Binary / primitive>: payload only
         if (is_key) return set_error(DFD_ERR_UNSUPPORTED, "column %lld (%s): list columns cannot be hash keys", i, name);
+        f->list = true;
+        f->kind = -1;
+        f->width = 0;
+        f->child_name = c->children[0]->name ? c->children[0]->name : "item";
+        f->child_format = c->children[0]->format;
+        f->child_flags = c->children[0]->flags;
         return DFD_OK;
     }
-    if (!c->format || !parse_format(c->format, &k, &w))
+    if (!c->format || !parse_format(c->format, &f->kind, &f->width))
         return set_error(DFD_ERR_UNSUPPORTED, "column %lld (%s): Arrow format '%s' is not supported", i, name, c->format ? c->format : "(null)");
+    f->view = c->format[0] == 'v';
     if (c->dictionary) {  // Dictionary<integer index, flat values>: indices are scattered, the dictionary travels by reference
-        if (k != DFD_COL_FIXED || !strchr("cCsSiIlL", c->format[0]) || c->format[1])
+        if (f->kind != DFD_COL_FIXED || !strchr("cCsSiIlL", c->format[0]) || c->format[1])
             return set_error(DFD_ERR_UNSUPPORTED, "column %lld (%s): dictionary index type '%s' is not an integer", i, name, c->format);
-        int32_t dk, dw;
         const ArrowSchema* d = c->dictionary;
-        if (d->dictionary || d->n_children > 0 || !d->format || !parse_format(d->format, &dk, &dw))
+        f->dict = true;
+        f->dict_index_unsigned = strchr("CSIL", c->format[0]) != nullptr;
+        f->dict_format = d->format ? d->format : "";
+        f->dict_flags = d->flags;
+        if (d->dictionary || d->n_children > 0 || !d->format || !parse_format(d->format, &f->dict_kind, &f->dict_width))
             return set_error(DFD_ERR_UNSUPPORTED, "column %lld (%s): dictionary value type '%s' is not supported", i, name, d->format ? d->format : "(null)");
         if (is_key && d->format[0] == 'v')
             return set_error(DFD_ERR_UNSUPPORTED, "column %lld (%s): dictionary KEY with view-typed values is not supported", i, name);
@@ -1523,8 +1682,10 @@ static int check_column(const ArrowSchema* c, long long i, bool is_key) {
 int dfd_schema_supported(const struct ArrowSchema* schema) {
     if (!schema || !schema->format || strcmp(schema->format, "+s") != 0)
         return set_error(DFD_ERR_INVALID_ARGUMENT, "schema must be a struct (record batch) schema");
-    for (int64_t i = 0; i < schema->n_children; ++i)
-        if (int rc = check_column(schema->children[i], (long long)i, false)) return rc;
+    for (int64_t i = 0; i < schema->n_children; ++i) {
+        FieldInfo f;
+        if (int rc = describe_column(schema->children[i], (long long)i, false, &f)) return rc;
+    }
     return DFD_OK;
 }
 
@@ -1537,7 +1698,8 @@ int dfd_repartition_supported(const struct ArrowSchema* schema, const int32_t* k
     for (int64_t i = 0; i < schema->n_children; ++i) {
         bool is_key = false;
         for (int k = 0; k < n_keys; ++k) is_key |= key_cols[k] == i;
-        if (int rc = check_column(schema->children[i], (long long)i, is_key)) return rc;
+        FieldInfo f;
+        if (int rc = describe_column(schema->children[i], (long long)i, is_key, &f)) return rc;
     }
     return DFD_OK;
 }
@@ -1549,54 +1711,16 @@ int dfd_repartition_exec_create(dfd_ctx* ctx, const struct ArrowSchema* schema, 
     if (!schema->format || strcmp(schema->format, "+s") != 0)
         return set_error(DFD_ERR_INVALID_ARGUMENT, "schema must be a struct (record batch) schema, got format '%s'",
                          schema->format ? schema->format : "(null)");
-    for (int64_t i = 0; i < schema->n_children; ++i) {  // (the same checks the plan hook runs through dfd_repartition_supported)
-        bool is_key = false;
-        for (int k = 0; k < n_keys; ++k) is_key |= key_cols && key_cols[k] == i;
-        if (int rc = check_column(schema->children[i], (long long)i, is_key)) return rc;
-    }
     std::unique_ptr<dfd_repartition_exec> x(new (std::nothrow) dfd_repartition_exec());
     if (!x) return set_error(DFD_ERR_OOM, "out of host memory");
     x->ctx = ctx;
     x->N = num_partitions;
-    for (int64_t i = 0; i < schema->n_children; ++i) {
-        const ArrowSchema* c = schema->children[i];
-        FieldInfo f;
-        f.name = c->name ? c->name : "";
-        f.format = c->format ? c->format : "";
-        f.flags = c->flags;
+    for (int64_t i = 0; i < schema->n_children; ++i) {  // (the same rules the plan hook checks through dfd_repartition_supported)
         int key_index = -1;
         for (int k = 0; k < n_keys; ++k)
             if (key_cols && key_cols[k] == i) key_index = k;
-        int32_t child_width = 0;
-        if (list_child_ok(c, &child_width)) {
-            if (key_index >= 0) return set_error(DFD_ERR_UNSUPPORTED, "column %lld (%s): list columns cannot be hash keys", (long long)i, f.name.c_str());
-            f.list = true;
-            f.child_width = child_width;
-            f.kind = -1;
-            f.width = 0;
-            f.child_name = c->children[0]->name ? c->children[0]->name : "item";
-            f.child_format = c->children[0]->format;
-            f.child_flags = c->children[0]->flags;
-            x->key_of_field.push_back(-1);
-            x->fields.push_back(f);
-            continue;
-        }
-        if (!parse_format(f.format.c_str(), &f.kind, &f.width))
-            return set_error(DFD_ERR_UNSUPPORTED, "column %lld (%s): Arrow format '%s' is not supported", (long long)i, f.name.c_str(), f.format.c_str());
-        f.view = f.format[0] == 'v';
-        if (c->dictionary) {
-            const ArrowSchema* d = c->dictionary;
-            if (f.kind != DFD_COL_FIXED || !strchr("cCsSiIlL", f.format[0]) || f.format[1])
-                return set_error(DFD_ERR_UNSUPPORTED, "column %lld (%s): dictionary index type '%s' is not an integer", (long long)i, f.name.c_str(), f.format.c_str());
-            f.dict = true;
-            f.dict_index_unsigned = strchr("CSIL", f.format[0]) != nullptr;
-            f.dict_format = d->format ? d->format : "";
-            f.dict_flags = d->flags;
-            if (d->dictionary || d->n_children > 0 || !parse_format(f.dict_format.c_str(), &f.dict_kind, &f.dict_width))
-                return set_error(DFD_ERR_UNSUPPORTED, "column %lld (%s): dictionary value type '%s' is not supported", (long long)i, f.name.c_str(), f.dict_format.c_str());
-            if (key_index >= 0 && f.dict_format[0] == 'v')
-                return set_error(DFD_ERR_UNSUPPORTED, "column %lld (%s): dictionary KEY with view-typed values is not supported", (long long)i, f.name.c_str());
-        }
+        FieldInfo f;
+        if (int rc = describe_column(schema->children[i], (long long)i, key_index >= 0, &f)) return rc;
         x->key_of_field.push_back(key_index);
         x->fields.push_back(f);
     }
@@ -1614,7 +1738,6 @@ int dfd_repartition_exec_create(dfd_ctx* ctx, const struct ArrowSchema* schema, 
             h.kind = DFD_COL_BINARY;
             h.width = 0;
             h.hidden = true;
-            h.owner = (int)i;
             h.role = tag[0] == 'l' ? 1 : tag[0] == 'b' ? 2 : 3;
             h.flags = nullable ? ARROW_FLAG_NULLABLE : 0;
             x->key_of_field.push_back(-1);
@@ -1625,14 +1748,14 @@ int dfd_repartition_exec_create(dfd_ctx* ctx, const struct ArrowSchema* schema, 
         x->fields[i].h_bytes = hidden("bytes", false);
         if (x->fields[i].child_flags & ARROW_FLAG_NULLABLE) x->fields[i].h_valid = hidden("validity", false);
     }
-    x->dev_pos.assign(x->fields.size(), -1);
+    std::vector<int> dev_pos(x->fields.size(), -1);  // field -> its position among the device columns
     for (size_t i = 0; i < x->fields.size(); ++i)
         if (!x->fields[i].nodev()) {
-            x->dev_pos[i] = (int)x->dev_fields.size();
+            dev_pos[i] = (int)x->dev_fields.size();
             x->dev_fields.push_back((int)i);
         }
     std::vector<int32_t> dev_keys(n_keys);
-    for (int k = 0; k < n_keys; ++k) dev_keys[k] = x->dev_pos[(size_t)key_cols[k]];  // keys address the compact device column list
+    for (int k = 0; k < n_keys; ++k) dev_keys[k] = dev_pos[(size_t)key_cols[k]];  // keys address the compact device column list
     int rc = dfd_partitioner_create(ctx, num_partitions, dev_keys.data(), n_keys, nullptr, &x->part);
     if (rc) return rc;  // (x has no CUDA resources yet; unique_ptr frees it)
     for (int k = 0; k < n_keys; ++k) {  // interval keys hash field by field (arrow's derived Hash), not as one integer
@@ -1656,43 +1779,9 @@ int dfd_repartition_exec_create(dfd_ctx* ctx, const struct ArrowSchema* schema, 
         e = cudaSetDevice(ctx->device);
         if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&x->s_h2d, cudaStreamNonBlocking);
         if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&x->s_d2h, cudaStreamNonBlocking);
-        const size_t C = x->fields.size();
         x->slots.resize(x->depth);
-        for (Slot& s : x->slots) {
-            s.d_in.assign(C, nullptr); s.d_in_valid.assign(C, nullptr); s.d_out.assign(C, nullptr); s.d_out_valid.assign(C, nullptr);
-            s.has_valid.assign(C, false);
-            s.h_valid.assign(C, nullptr); s.h_bool.assign(C, nullptr); s.h_off.assign(C, nullptr); s.dict_id.assign(C, DictId{});
-            s.d_in_off.assign(C, nullptr); s.d_out_off.assign(C, nullptr);
-            s.in_cap.assign(C, 0); s.out_cap.assign(C, 0);
-            s.first_off.assign(C, 0); s.data_bytes.assign(C, 0);
-            s.dict_buf.resize(C); s.dict_hashes.assign(C, nullptr); s.dict_valid.assign(C, nullptr);
-            s.list_tmp.resize(C);
-            for (size_t i = 0; i < C && e == cudaSuccess; ++i) {
-                const FieldInfo& f = x->fields[i];
-                if (f.nodev()) continue;  // list placeholder: its rows live in the hidden columns
-                if (f.var()) {  // offsets now, string bytes on demand
-                    e = cudaMalloc(&s.d_in_off[i], (size_t)(x->chunk_rows + 16) * f.ow());
-                    if (e == cudaSuccess) e = cudaHostAlloc((void**)&s.h_off[i], (size_t)(x->chunk_rows + 16) * f.ow(), cudaHostAllocPortable);
-                    if (e == cudaSuccess) e = cudaMalloc(&s.d_out_off[i], (size_t)(x->chunk_rows + 16) * f.ow());
-                    if (e == cudaSuccess && (f.flags & ARROW_FLAG_NULLABLE)) {
-                        e = cudaMalloc(&s.d_in_valid[i], PinnedPool::bitmap_bytes(x->chunk_rows) + 8);
-                        if (e == cudaSuccess) e = cudaMalloc(&s.d_out_valid[i], PinnedPool::bitmap_bytes(x->chunk_rows) + 8);
-                    }
-                    continue;
-                }
-                size_t vb = PinnedPool::value_bytes(f, x->chunk_rows) + 16 * (size_t)(f.width ? f.width : 1);
-                e = cudaMalloc(&s.d_in[i], vb);
-                if (e == cudaSuccess) e = cudaMalloc(&s.d_out[i], vb);
-                if (e == cudaSuccess && (f.flags & ARROW_FLAG_NULLABLE)) {
-                    e = cudaMalloc(&s.d_in_valid[i], PinnedPool::bitmap_bytes(x->chunk_rows) + 8);
-                    if (e == cudaSuccess) e = cudaMalloc(&s.d_out_valid[i], PinnedPool::bitmap_bytes(x->chunk_rows) + 8);
-                }
-            }
-            if (e == cudaSuccess) e = cudaHostAlloc((void**)&s.h_part_starts, sizeof(int64_t) * (num_partitions + 1), cudaHostAllocPortable);
-            if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s.e_h2d, cudaEventDisableTiming);
-            if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s.e_k, cudaEventDisableTiming);
-            if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s.e_d2h, cudaEventDisableTiming);
-        }
+        for (Slot& s : x->slots)
+            if (e == cudaSuccess) e = alloc_slot(x.get(), s);
     }
     if (e != cudaSuccess) {
         int code = cuda_error(e, "dfd_repartition_exec_create allocations");
@@ -1716,11 +1805,7 @@ int dfd_repartition_exec_create(dfd_ctx* ctx, const struct ArrowSchema* schema, 
         pre.push_back(c);
     }
     for (OutChunk* c : pre) x->pool->give_back(c);
-    x->tmp_off.resize(x->fields.size());
-    x->tmp_bytes.resize(x->fields.size());
-    x->prep.resize(x->fields.size());
-    x->view_tmp.resize(x->fields.size());
-    x->dsz.assign(x->fields.size(), std::vector<int64_t>(4, 0));
+    x->tmp.resize(x->fields.size());
     x->cur = x->depth - 1;  // open_next_slot() starts at slot 0
     *out = x.release();
     return DFD_OK;
@@ -1735,29 +1820,10 @@ void dfd_repartition_exec_destroy(dfd_repartition_exec* x) {
         if (x->s_d2h) cudaStreamSynchronize(x->s_d2h);
         cudaStreamSynchronize(x->ctx->stream);
         cudaFree(x->d_sizes.ptr);
-        for (dfd::Scratch& b : x->view_tmp) cudaFree(b.ptr);
+        for (FieldTmp& t : x->tmp) cudaFree(t.view_dev.ptr);
         if (x->h_sizes) cudaFreeHost(x->h_sizes);
         if (x->e_sizes) cudaEventDestroy(x->e_sizes);
-        for (Slot& s : x->slots) {
-            s.held.clear();
-            s.dict_held.clear();
-            if (s.out) { s.out->refs.store(1); s.out->pool = x->pool; chunk_unref(s.out); }
-            for (void* p : s.d_in) cudaFree(p);
-            for (void* p : s.d_in_valid) cudaFree(p);
-            for (void* p : s.d_out) cudaFree(p);
-            for (void* p : s.d_out_valid) cudaFree(p);
-            for (void* p : s.d_in_off) cudaFree(p);
-            for (void* p : s.d_out_off) cudaFree(p);
-            for (uint8_t* p : s.h_valid) if (p) cudaFreeHost(p);
-            for (uint8_t* p : s.h_bool) if (p) cudaFreeHost(p);
-            for (char* p : s.h_off) if (p) cudaFreeHost(p);
-            for (dfd::Scratch& b : s.dict_buf) cudaFree(b.ptr);
-            for (dfd::Scratch& b : s.list_tmp) cudaFree(b.ptr);
-            if (s.h_part_starts) cudaFreeHost(s.h_part_starts);
-            if (s.e_h2d) cudaEventDestroy(s.e_h2d);
-            if (s.e_k) cudaEventDestroy(s.e_k);
-            if (s.e_d2h) cudaEventDestroy(s.e_d2h);
-        }
+        for (Slot& s : x->slots) free_slot(x, s);
         if (x->s_h2d) cudaStreamDestroy(x->s_h2d);
         if (x->s_d2h) cudaStreamDestroy(x->s_d2h);
     }
@@ -1771,137 +1837,22 @@ void dfd_repartition_exec_destroy(dfd_repartition_exec* x) {
 int dfd_repartition_exec_push(dfd_repartition_exec* x, struct ArrowArray* batch) {
     if (!x || !batch) return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_repartition_exec_push: NULL argument");
     ScopedNs timed(x->ns_push);
-    auto drop = [&]() { if (batch->release) batch->release(batch); };
-    if (x->finished) { drop(); return set_error(DFD_ERR_INVALID_ARGUMENT, "push after finish/error: %s", x->error.c_str()); }
-    if (batch->n_children != (int64_t)x->n_visible) {
-        drop();
-        return fail(x, DFD_ERR_INVALID_ARGUMENT, "batch has " + std::to_string(batch->n_children) + " columns, schema has " + std::to_string(x->n_visible));
-    }
-    const int64_t R = batch->length;
-    x->rows_in += (uint64_t)R;
-    if (R == 0) { drop(); return DFD_OK; }
-    if (x->input_mode == INPUT_DEVICE) {
-        drop();
-        const int rc = fail(x, DFD_ERR_INVALID_ARGUMENT, "host batch pushed to an operator that takes device batches (push_device)");
-        release_device_inputs(x);
-        return rc;
-    }
-    for (int64_t i = 0; i < batch->n_children; ++i)
-        if (batch->children[i]->length < R || (batch->offset != 0)) {
-            drop();
-            return fail(x, DFD_ERR_INVALID_ARGUMENT, "record batch children shorter than the batch, or non-zero struct offset");
-        }
-    x->input_mode = INPUT_HOST;
-    // ownership of the batch moves to a shared holder: every chunk that stages rows from it (and, for dictionary columns,
-    // every output batch that references its dictionaries) keeps it alive
-    HeldInput holder = std::make_shared<SharedInput>(*batch);
-    batch->release = nullptr;
-    const ArrowArray* in = &holder->array;
-    int rc = DFD_OK;
-    int64_t done = 0;
-    while (done < R) {
-        if (!x->cur_open && (rc = open_next_slot(x))) return rc;
-        Slot& s = x->slots[x->cur];
-        const int64_t room = x->chunk_rows - s.rows;
-        if (room == 0) {
-            if ((rc = flush_current(x))) return rc;
-            continue;
-        }
-        const int64_t n = R - done < room ? R - done : room;
-        // batches of every shape are APPENDED to the open chunk (bitmaps concatenated at bit granularity, string offsets
-        // re-based); the chunk is cut early only when these rows cannot join it: another dictionary, or string bytes beyond
-        // what 32-bit offsets address
-        bool fits = true;
-        if ((rc = prepare_rows(x, in, done, n, &fits))) return rc;
-        if (!fits) {
-            if ((rc = flush_current(x))) return rc;
-            continue;  // (prepared again against an empty chunk, which always fits or grows)
-        }
-        if ((rc = stage_rows(x, in, done, n))) return rc;
-        s.held.push_back(holder);
-        done += n;
-        if (s.rows == x->chunk_rows && (rc = flush_current(x))) return rc;
-    }
-    return emit_ready(x);
+    if (x->finished) return refuse_after_finish(x, batch);
+    return push_rows(x, batch, INPUT_HOST, nullptr);
 }
 
 int dfd_repartition_exec_push_device(dfd_repartition_exec* x, struct ArrowDeviceArray* batch) {
     if (!x || !batch) return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_repartition_exec_push_device: NULL argument");
     ScopedNs timed(x->ns_push);
     ArrowArray* a = &batch->array;
-    auto drop = [&]() { if (a->release) a->release(a); };
-    if (x->finished) { drop(); return set_error(DFD_ERR_INVALID_ARGUMENT, "push after finish/error: %s", x->error.c_str()); }
-    auto refuse = [&](int code, const std::string& msg) {  // the batch is released, the operator fails (and lets go of earlier batches)
-        drop();
-        const int rc = fail(x, code, msg);
-        if (x->input_mode == INPUT_DEVICE) release_device_inputs(x);
-        return rc;
-    };
+    if (x->finished) return refuse_after_finish(x, a);
     if (!launch_stage_batch || !launch_stage_sizes)  // (weak: see dfd_internal.h)
-        return refuse(DFD_ERR_UNSUPPORTED, "device input: this build of the operator has no staging kernels (dfd_stage.cu)");
+        return refuse(x, a, DFD_ERR_UNSUPPORTED, "device input: this build of the operator has no staging kernels (dfd_stage.cu)");
     if (batch->device_type != ARROW_DEVICE_CUDA || batch->device_id != (int64_t)x->ctx->device)
-        return refuse(DFD_ERR_INVALID_ARGUMENT, "device batch of device type " + std::to_string((int)batch->device_type) + ", device " +
-                                                    std::to_string(batch->device_id) + ": the operator takes CUDA batches of device " +
-                                                    std::to_string(x->ctx->device));
-    if (a->n_children != (int64_t)x->n_visible)
-        return refuse(DFD_ERR_INVALID_ARGUMENT, "batch has " + std::to_string(a->n_children) + " columns, schema has " + std::to_string(x->n_visible));
-    const int64_t R = a->length;
-    x->rows_in += (uint64_t)R;
-    if (R == 0) { drop(); return DFD_OK; }
-    if (x->input_mode == INPUT_HOST)
-        return refuse(DFD_ERR_INVALID_ARGUMENT, "device batch pushed to an operator that takes host batches (push / run)");
-    for (int64_t i = 0; i < a->n_children; ++i)
-        if (a->children[i]->length < R || (a->offset != 0))
-            return refuse(DFD_ERR_INVALID_ARGUMENT, "record batch children shorter than the batch, or non-zero struct offset");
-    x->input_mode = INPUT_DEVICE;
-    if (batch->sync_event) {  // the staging stream waits for the producer's work; the host does not
-        cudaError_t e;
-        {
-            std::lock_guard<std::mutex> lk(x->ctx->mu);
-            e = cudaSetDevice(x->ctx->device);
-            if (e == cudaSuccess) e = cudaStreamWaitEvent(x->s_h2d, *(cudaEvent_t*)batch->sync_event, 0);
-        }
-        if (e != cudaSuccess) return refuse(DFD_ERR_CUDA, std::string("wait on the batch's sync_event: ") + cudaGetErrorString(e));
-    }
-    // ownership moves to a shared holder, as in push(): released once the chunks that read it have been emitted
-    HeldInput holder = std::make_shared<SharedInput>(*a);
-    a->release = nullptr;
-    const ArrowArray* in = &holder->array;
-    auto bail = [&](int rc) {
-        release_device_inputs(x);
-        return rc;
-    };
-    int rc = DFD_OK;
-    HeldInput dicts;
-    for (const FieldInfo& f : x->fields)
-        if (f.dict) {
-            if ((rc = host_dictionaries(x, in, &dicts))) return bail(rc);
-            break;
-        }
-    int64_t done = 0;
-    while (done < R) {
-        if (!x->cur_open && (rc = open_next_slot(x))) return bail(rc);
-        Slot& s = x->slots[x->cur];
-        const int64_t room = x->chunk_rows - s.rows;
-        if (room == 0) {
-            if ((rc = flush_current(x))) return bail(rc);
-            continue;
-        }
-        const int64_t n = R - done < room ? R - done : room;
-        bool fits = true;
-        if ((rc = prepare_rows_device(x, in, dicts, done, n, &fits))) return bail(rc);
-        if (!fits) {
-            if ((rc = flush_current(x))) return bail(rc);
-            continue;
-        }
-        if ((rc = stage_rows_device(x, in, dicts, done, n))) return bail(rc);
-        s.held.push_back(holder);
-        if (dicts) s.dict_held.push_back(dicts);
-        done += n;
-        if (s.rows == x->chunk_rows && (rc = flush_current(x))) return bail(rc);
-    }
-    if ((rc = emit_ready(x))) return bail(rc);
-    return DFD_OK;
+        return refuse(x, a, DFD_ERR_INVALID_ARGUMENT, "device batch of device type " + std::to_string((int)batch->device_type) + ", device " +
+                                                          std::to_string(batch->device_id) + ": the operator takes CUDA batches of device " +
+                                                          std::to_string(x->ctx->device));
+    return push_rows(x, a, INPUT_DEVICE, batch->sync_event);
 }
 
 int dfd_repartition_exec_finish(dfd_repartition_exec* x) {

@@ -2,7 +2,9 @@
 supported column kind — fixed widths, nullable, boolean, Utf8 / LargeUtf8 / Binary, views, dictionaries (changing between
 batches, null values, null indices), List<Utf8 / Binary> — as payload and, where allowed, as hash key; ragged and sliced
 input batches against chunk sizes that cut them anywhere.  Every destination must hold the rows the oracle's partition
-ids select, in input order, with the input schema."""
+ids select, in input order, with the input schema.  Every case runs twice: host batches through push, and the same batches
+as device batches (host stand-ins, tests/device_batches.py) through push_device on the device harness library
+(tests/test_exec_device_input_cpu_harness.py), a superset of the host one."""
 import random
 
 import numpy as np
@@ -10,7 +12,8 @@ import pyarrow as pa
 import pytest
 
 from oracle import oracle as orc
-from tests.test_exec_cpu_harness import harness  # noqa: F401  (module-scoped fixture: builds the harness once)
+from tests import device_batches as DB
+from tests.test_exec_device_input_cpu_harness import harness  # noqa: F401  (module-scoped fixture: builds the harness once)
 from tests.util import expected_partitions
 
 
@@ -118,7 +121,7 @@ KINDS = ["i64", "i32?", "u8", "f64", "bool?", "date32", "dec128?", "utf8?", "lar
 
 @pytest.mark.parametrize("seed", range(24))
 def test_random_schema_and_batching_matches_the_oracle(harness, seed):  # noqa: F811
-    ns, ctx = harness
+    ns, ctx, _ = harness
     rnd = random.Random(1000 + seed)
     rng = np.random.Generator(np.random.PCG64(1000 + seed))
     n = rnd.choice([1, 63, 1000, 5000, 20_000])
@@ -137,40 +140,47 @@ def test_random_schema_and_batching_matches_the_oracle(harness, seed):  # noqa: 
     keys = rnd.sample(keyable, rnd.randint(1, min(3, len(keyable))))
     N = rnd.choice([1, 2, 3, 8, 12, 48, 257])
     chunk_rows = rnd.choice([64, 1000, 4096, 0])
-    ex = ns.RepartitionExec(ctx, fed.schema, ns.Partitioning.Hash(keys, N), chunk_rows=chunk_rows, pipeline_depth=rnd.choice([0, 2, 4]))
+    depth = rnd.choice([0, 2, 4])
     # ragged feeding: random cuts, each cut re-batched with a random maximum size (slices with odd offsets, empty batches)
     cuts = sorted({0, n} | {rnd.randint(0, n) for _ in range(rnd.randint(0, 6))})
+    batches = []
     for a, b in zip(cuts[:-1], cuts[1:]):
-        for rb in fed.slice(a, b - a).to_batches(max_chunksize=rnd.choice([7, 100, 8192, 100_000])):
-            ex.push_batch(rb)
+        batches += fed.slice(a, b - a).to_batches(max_chunksize=rnd.choice([7, 100, 8192, 100_000]))
     if rnd.random() < 0.3:
-        ex.push_batch(fed.slice(0, 0).to_batches()[0] if fed.slice(0, 0).to_batches() else pa.RecordBatch.from_pylist([], schema=fed.schema))
-    ex.finish()
-    outs = [ex.execute(p).read_all() for p in range(N)]
-    st = ex.stats()
-    assert st["rows_in"] == n and st["rows_out"] == n
+        batches.append(fed.slice(0, 0).to_batches()[0] if fed.slice(0, 0).to_batches() else pa.RecordBatch.from_pylist([], schema=fed.schema))
     dest = orc.partition_ids([plain.column(k) for k in keys], n, N)
     order, starts = expected_partitions(dest, N)
-    for p in range(N):
-        want = plain.take(pa.array(order[starts[p]:starts[p + 1]]))
-        got = outs[p]
-        assert got.schema.equals(fed.schema), (kinds, p)
-        assert got.num_rows == want.num_rows, (kinds, keys, N, p)
-        if got.num_rows:
-            got.validate(full=True)
-        for name in names:
-            g, w = got.column(name), want.column(name).combine_chunks()
-            if pa.types.is_dictionary(g.type):  # decode chunk by chunk (the chunks of a destination may carry different dictionaries)
-                g = pa.chunked_array([c.dictionary_decode() for c in g.chunks], type=g.type.value_type)
-            g = g.combine_chunks()
-            assert g.cast(w.type).equals(w), (kinds, keys, N, chunk_rows, p, name)
-    ex.close()
+    for device in (False, True):
+        ex = ns.RepartitionExec(ctx, fed.schema, ns.Partitioning.Hash(keys, N), chunk_rows=chunk_rows, pipeline_depth=depth)
+        for rb in batches:
+            if device:
+                ex.push_device_batch(DB.DeviceBatch(rb, alloc=DB.host_alloc).device_array)
+            else:
+                ex.push_batch(rb)
+        ex.finish()
+        outs = [ex.execute(p).read_all() for p in range(N)]
+        st = ex.stats()
+        assert st["rows_in"] == n and st["rows_out"] == n
+        for p in range(N):
+            want = plain.take(pa.array(order[starts[p]:starts[p + 1]]))
+            got = outs[p]
+            assert got.schema.equals(fed.schema), (kinds, p, device)
+            assert got.num_rows == want.num_rows, (kinds, keys, N, p, device)
+            if got.num_rows:
+                got.validate(full=True)
+            for name in names:
+                g, w = got.column(name), want.column(name).combine_chunks()
+                if pa.types.is_dictionary(g.type):  # decode chunk by chunk (the chunks of a destination may carry different dictionaries)
+                    g = pa.chunked_array([c.dictionary_decode() for c in g.chunks], type=g.type.value_type)
+                g = g.combine_chunks()
+                assert g.cast(w.type).equals(w), (kinds, keys, N, chunk_rows, p, name, device)
+        ex.close()
 
 
 def test_long_strings_grow_the_chunk_buffers(harness):  # noqa: F811
     """Strings of tens of kilobytes (a plain column, a view column and the elements of a list): the chunk's device byte
     buffers and the pinned landing buffers grow while batches are appended, without losing what is already staged."""
-    ns, ctx = harness
+    ns, ctx, _ = harness
     rnd = random.Random(3)
     n, N = 1500, 5
     big = pa.array([None if rnd.random() < 0.05 else ("x" * rnd.choice([0, 10, 3000, 20000]) + str(i)) for i in range(n)], type=pa.string())

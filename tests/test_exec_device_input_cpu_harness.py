@@ -134,6 +134,53 @@ def test_device_input_leaves_no_allocation_behind(harness, monkeypatch):
     assert lib.harness_live_allocations() == base
 
 
+@pytest.mark.parametrize("what,name", [(0, "cudaMalloc"), (1, "cudaHostAlloc"), (2, "cudaMemcpyAsync")])
+def test_injected_cuda_failures_on_device_input_surface_as_errors_and_leak_nothing(harness, what, name):
+    """The device-input counterpart of test_exec_cpu_harness.py::test_injected_cuda_failures_surface_as_errors_and_leak_nothing:
+    fail the n-th cudaMalloc / cudaHostAlloc / cudaMemcpyAsync of an operator fed device batches (create, sizes read-back,
+    dictionary copies, staging, flush, D2H).  The failure comes back as an error, never a crash; once everything is closed
+    no allocation is left behind, and every pushed batch has been released exactly once."""
+    import gc
+
+    import pyarrow as pa
+
+    from tests import device_batches as DB
+    from tests.test_exec_cpu_harness import _fixture_like_table
+
+    ns, hctx, _ = harness
+    lib = hctx.lib
+    lib.harness_live_allocations.restype = C.c_long
+    lib.harness_fail_nth.argtypes = [C.c_int, C.c_long]
+    batches = _fixture_like_table(1500).to_batches(max_chunksize=500)
+    failures = 0
+    for n in list(range(1, 40)) + [60, 90, 150, 400]:
+        base = lib.harness_live_allocations()
+        ctx = _Ctx(lib)
+        lib.harness_fail_nth(what, n)
+        ex, pushed = None, []
+        try:
+            ex = ns.RepartitionExec(ctx, batches[0].schema, ns.Partitioning.Hash([4, 0], 4), chunk_rows=512)
+            for rb in batches:
+                b = DB.DeviceBatch(rb, alloc=DB.host_alloc)
+                pushed.append(b.key)
+                ex.push_device_batch(b.device_array)
+            ex.finish()
+            assert sum(ex.execute(p).read_all().num_rows for p in range(4)) == 1500  # (the failing call was not on this path)
+        except (ns.DfdError, pa.ArrowException, OSError) as e:
+            failures += 1
+            assert "fake CUDA" in str(e) or "failed" in str(e) or "alloc" in str(e).lower() or "cuda" in str(e).lower(), str(e)
+        finally:
+            lib.harness_fail_nth(what, 0)
+            if ex is not None:
+                ex.close()
+            ctx.close()
+            gc.collect()
+        assert not set(pushed) & DB.live_batches(), (name, n)
+        assert sorted(k for k in DB.RELEASED if k in set(pushed)) == sorted(pushed), (name, n)  # each exactly once
+        assert lib.harness_live_allocations() == base, (name, n)
+    assert failures >= 5, (name, failures)
+
+
 def test_an_operator_object_linked_without_the_staging_kernels_refuses_device_batches(built, tmp_path):
     """The host-logic harness WITHOUT harness_stage.cu: the operator object still loads (its references to the staging
     launches are weak), host batches work as ever, and a device batch is refused with DFD_ERR_UNSUPPORTED and released."""

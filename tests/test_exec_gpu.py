@@ -140,6 +140,22 @@ def test_operator_errors(ctx):
         with pytest.raises(Exception):
             ex.execute(p).read_all()
     ex.close()
+    # a List<Utf8> whose child offsets decrease over the pushed rows (list offsets 1, 1, 2 over child offsets 0, 6, 2, 8: the
+    # rows' element runs from byte 6 to byte 2): refused before any of its bytes are staged, and the error reaches every
+    # partition stream
+    child = pa.Array.from_buffers(pa.string(), 3, [None, pa.py_buffer(np.array([0, 6, 2, 8], dtype=np.int32).tobytes()), pa.py_buffer(b"abcdefgh")])
+    lst = pa.Array.from_buffers(pa.list_(pa.string()), 2, [None, pa.py_buffer(np.array([1, 1, 2], dtype=np.int32).tobytes())], children=[child])
+    rb = pa.RecordBatch.from_arrays([pa.array([1, 2], type=pa.int64()), lst], names=["k", "s"])
+    ex = dfd.RepartitionExec(ctx, rb.schema, dfd.Partitioning.Hash([0], 2))
+    with pytest.raises(dfd.DfdError) as e:
+        ex.push_batch(rb)
+    assert e.value.status == 1 and "list offsets are not monotonic" in str(e.value)  # DFD_ERR_INVALID_ARGUMENT
+    with pytest.raises(dfd.DfdError):
+        ex.finish()
+    for p in range(2):
+        with pytest.raises(Exception):
+            ex.execute(p).read_all()
+    ex.close()
 
 
 def test_abort_fails_every_partition_stream_after_the_queued_rows(ctx):
