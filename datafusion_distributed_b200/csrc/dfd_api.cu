@@ -128,9 +128,9 @@ static int build_keyset(const dfd_partitioner* p, const dfd_column* cols, int n_
         if (_e != cudaSuccess) return cuda_error(_e, what);            \
     }
 
-// Aligned write-out costs local HBM stores more write-out iterations (L2 already merges partial lines)
-// but gives NVLink peer stores full-size write packets, so it is on for the fused exchange only.
-// DFD_ALIGNED_WRITEOUT=0/1 forces it.
+// Aligned write-out gives NVLink peer stores full-size write packets, so it is on for the fused exchange only.
+// A local single-pass launch aligns its stores without it (its KV == K write-out stores warp-aligned output-row
+// pairs, see k_scatter_onepass).  DFD_ALIGNED_WRITEOUT=0/1 forces it.
 bool dfd::use_aligned(uint32_t N, bool peer) {
     static const int forced = [] { const char* e = getenv("DFD_ALIGNED_WRITEOUT"); return e ? (atoi(e) != 0 ? 1 : 0) : -1; }();
     if (N > ALIGNED_MAX_N) return false;

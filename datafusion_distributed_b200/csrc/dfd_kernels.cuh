@@ -301,11 +301,21 @@ struct StageIO {
 };
 
 constexpr uint32_t SLOT_NONE = 0xffffffffu;
+// up to this many destinations the single-pass local write-out aligns every warp's pairs to 32 pairs (= ALIGNED_MAX_N)
+constexpr uint32_t PAIR_ALIGN_MAX_N = 16;
 
 // Payload columns are streamed exactly once: evict-first loads / stores keep the L2 for what is reused
 // (the key tiles between phase 1 and the scatter of the same tile, the look-back descriptors).
 template <typename V> __device__ __forceinline__ V ld_stream(const V* p) { return __ldcs(p); }
 template <typename V> __device__ __forceinline__ void st_stream(V* p, V v) { __stcs(p, v); }
+// p[0] = a, p[1] = b as one streaming store (p aligned to 2 * sizeof(V))
+template <typename V> __device__ __forceinline__ void st_stream_pair(V* p, V a, V b) {
+    static_assert(sizeof(V) <= 8, "two values of at most 8 bytes");
+    if constexpr (sizeof(V) == 8) __stcs((ulonglong2*)p, make_ulonglong2(a, b));
+    else if constexpr (sizeof(V) == 4) __stcs((uint2*)p, make_uint2(a, b));
+    else if constexpr (sizeof(V) == 2) __stcs((unsigned*)p, (unsigned)a | ((unsigned)b << 16));
+    else __stcs((unsigned short*)p, (unsigned short)((unsigned)a | ((unsigned)b << 8)));
+}
 
 // ROWS == false: slot[k] = (destination << 16 | staging index) for write-out iteration k (or SLOT_NONE)
 // ROWS == true : slot[k] = absolute output row of staging index k*THREADS + threadIdx.x (or SLOT_NONE) — local
@@ -677,7 +687,7 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src, uint32
 
 // shared-memory layout of k_scatter_onepass
 struct OnePassSmem {
-    uint32_t off_bars, off_tix, off_delta, off_ob, off_wc, off_ts, off_scan, off_misc, off_vs, off_src, off_d8, total;
+    uint32_t off_bars, off_tix, off_delta, off_ob, off_wc, off_ts, off_scan, off_misc, off_vs, off_src, total;
 };
 // S: ring items per column of a tile (each one a range of T / S rows), so a slot holds T * width / S bytes
 template <int THREADS, int K, int NB, int S>
@@ -693,10 +703,9 @@ __host__ __device__ __forceinline__ OnePassSmem onepass_smem_layout(uint32_t N, 
     L.off_ts = L.off_wc + W * N * 4u;
     L.off_scan = L.off_ts + 2u * (N + 1u) * 4u;
     L.off_misc = L.off_scan + (W + 1u) * 4u;
-    L.off_vs = L.off_misc + 4u * 4u;                          // aligned mode: virtual run starts
-    L.off_src = (L.off_vs + (aligned ? (N + 1u) * 4u : 0u) + 3u) & ~3u;
-    L.off_d8 = L.off_src + 2u * T * 2u;
-    L.total = L.off_d8 + 2u * T;
+    L.off_vs = L.off_misc + 4u * 4u;                          // aligned mode: virtual run starts; local row mode: pair starts
+    L.off_src = (L.off_vs + (aligned || !peer ? (N + 1u) * 4u : 0u) + 3u) & ~3u;
+    L.total = L.off_src + 2u * T * 2u;
     return L;
 }
 
@@ -774,7 +783,8 @@ __device__ __forceinline__ void onepass_by_width(int cw, int parts, F&& f) {
 //        tiles' descriptors, 32 predecessors per step.  Because phase 1 of a tile runs a whole tile-time
 //        before its look-back, the aggregates below it are always published already;
 //      scatter: per column item, slot i of the destination order is gathered from the ring (src row) and
-//        stored to its output row — consecutive threads write consecutive rows of a destination's run.
+//        stored to its output row — consecutive threads write consecutive rows of a destination's run; local
+//        launches with KV == K write two output rows per store (pairs on even output rows, warp-aligned for small N).
 // Order is stable (cursor = sum over lower tiles).  Destinations live in fixed regions (dest_base /
 // region_stride); a tile that would overflow a region sets overflow_out and writes nothing — the counts stay
 // exact and the host re-runs with exact regions.
@@ -948,7 +958,6 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
         const int tile_rows = (int)((P.n_rows - row0) < T ? (P.n_rows - row0) : T);
         uint32_t* const TS = (uint32_t*)(smem + L.off_ts) + (uint32_t)buf * (N + 1u);
         uint16_t* const SRC16 = (uint16_t*)(smem + L.off_src) + (uint32_t)buf * T;
-        uint8_t* const DEST8 = smem + L.off_d8 + (uint32_t)buf * T;
         uint32_t* wc = WARP_CNT + (uint32_t)w * N;
         for (uint32_t p = lane; p < N; p += 32) wc[p] = 0;
         __syncwarp();
@@ -1005,11 +1014,7 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
 #pragma unroll
         for (int j = 0; j < K; ++j) {
             const uint32_t d = pos[j] >> 16;
-            if (d < N) {
-                const uint32_t sp = wc[d] + (pos[j] & 0xffffu);  // slot of this row in destination order
-                SRC16[sp] = (uint16_t)(t0 + j * 32);
-                DEST8[sp] = (uint8_t)d;  // N <= 256 in single-pass mode
-            }
+            if (d < N) SRC16[wc[d] + (pos[j] & 0xffffu)] = (uint16_t)(t0 + j * 32);  // slot of this row in destination order
         }
         DFD_CLK_ADD(clk_on, CLK_PHASE1, clk_p1);
         return tile;
@@ -1039,7 +1044,7 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
         DFD_CLK_COUNT(clk_on, CLK_TILES);
         DFD_CLK_START(clk_lb);
         if (threadIdx.x == 0) S_MISC[0] = 0;
-        block_sync<THREADS, BAR>();  // (also: SRC16 / DEST8 of this tile are visible, DELTA is free)
+        block_sync<THREADS, BAR>();  // (also: SRC16 of this tile is visible, DELTA is free)
         // ---- decoupled look-back: exclusive prefix of every destination over the lower tiles
         // (a warp owns destinations w, w+W, ...: the first window of predecessor descriptors is loaded for LBQ of them at once,
         //  so their L2 round trips overlap instead of queueing behind each other — with N = 48 that is 6 per warp)
@@ -1101,16 +1106,60 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
         const bool overflow = S_MISC[0] != 0;
         if (overflow && threadIdx.x == 0) *P.overflow_out = 1;  // a region is too small: this tile writes nothing
         const uint16_t* const SRC16 = (const uint16_t*)(smem + L.off_src) + (uint32_t)buf * T;
-        const uint8_t* const DEST8 = smem + L.off_d8 + (uint32_t)buf * T;
         if constexpr (ROWS) {
-            // absolute output row (< 2^32: host-checked) and source row of every slot this thread writes
-            uint32_t orow[K], src[K];
+            // Output-row pairs: destination p's run [o, o + cnt) of absolute output rows (o = TS[p] + DELTA[p]; o + cnt < 2^32 - 1,
+            // host-checked) is cut on even output rows into ((o + cnt - 1) >> 1) - (o >> 1) + 1 pairs, so a full pair is one
+            // aligned store of two rows and only an odd head row or an odd tail row of a run is stored alone.  With at most
+            // PAIR_ALIGN_MAX_N destinations each run of pairs is also padded in front by (o >> 1) mod 32 pairs and rounded up to
+            // 32, so every warp store covers one aligned 32-pair span (512 B for 8-byte values): at most T / 2 + 63 N pairs.
+            // Above that bound, pairs only: at most T / 2 + N, N <= 256 in single-pass mode.  Pair v of the tile is virtual
+            // pair v - VP[p] of destination p; consecutive threads take consecutive pairs.
+            constexpr int KP = (T / 2 + (63 * PAIR_ALIGN_MAX_N > 256 ? 63 * PAIR_ALIGN_MAX_N : 256) + THREADS - 1) / THREADS;
+            static_assert(T <= 0x8000, "a pair packs 15-bit source rows");
+            const uint32_t wmask = N <= PAIR_ALIGN_MAX_N ? 31u : 0u;
+            uint32_t* const VP = (uint32_t*)(smem + L.off_vs);
+            {
+                uint32_t carry = 0;
+                for (uint32_t p0 = 0; p0 < N; p0 += THREADS) {
+                    const uint32_t p = p0 + threadIdx.x;
+                    uint32_t np = 0;
+                    if (p < N) {
+                        const uint32_t cnt = TS[p + 1] - TS[p], o = (uint32_t)(DELTA[p] + (int64_t)TS[p]);
+                        np = cnt ? ((((o + cnt - 1u) >> 1) - (o >> 1) + 1u + ((o >> 1) & wmask)) + wmask) & ~wmask : 0u;
+                    }
+                    uint32_t tot;
+                    const uint32_t ex = block_exclusive_scan<THREADS, BAR>(np, S_SCAN, tot);
+                    if (p < N) VP[p] = carry + ex;
+                    carry += tot;
+                }
+                if (threadIdx.x == 0) VP[N] = carry;
+                block_sync<THREADS, BAR>();
+            }
+            // per pair: its first live output row (SLOT_NONE: none) and source rows (bits 0-14: that row's, bit 15: the next
+            // output row is live too, bits 16-31: its source row); tile rows < 2^15
+            uint32_t orow[KP], src[KP];
+            const uint32_t n_pairs = overflow ? 0u : VP[N];
 #pragma unroll
-            for (int k = 0; k < K; ++k) {
-                const uint32_t i = k * THREADS + threadIdx.x;
-                const bool on = i < (uint32_t)tile_rows && !overflow;
-                orow[k] = on ? i + (uint32_t)DELTA[DEST8[i]] : SLOT_NONE;
-                src[k] = on ? SRC16[i] : 0;
+            for (int k = 0; k < KP; ++k) {
+                const uint32_t v = k * THREADS + threadIdx.x;
+                orow[k] = SLOT_NONE;
+                src[k] = 0;
+                if (v < n_pairs) {
+                    uint32_t lo = 0, hi = N;  // last p with VP[p] <= v
+                    while (hi - lo > 1) {
+                        const uint32_t mid = (lo + hi) >> 1;
+                        if (VP[mid] <= v) lo = mid; else hi = mid;
+                    }
+                    const uint32_t ts = TS[lo], cnt = TS[lo + 1] - ts, o = (uint32_t)(DELTA[lo] + (int64_t)ts);
+                    const uint32_t q = v - VP[lo] - ((o >> 1) & wmask);  // pair of the run (wraps in the leading pad)
+                    if (q > ((o + cnt - 1u) >> 1) - (o >> 1)) continue;  // padding
+                    const uint32_t pr = ((o >> 1) + q) << 1;  // even output row of the pair (<= o + cnt - 1: no wrap)
+                    const uint32_t first = pr < o ? o : pr;
+                    const uint32_t i = ts + (first - o);  // its slot in destination order
+                    orow[k] = first;
+                    src[k] = SRC16[i];
+                    if (first == pr && pr + 1u - o < cnt) src[k] |= 0x8000u | ((uint32_t)SRC16[i + 1] << 16);
+                }
             }
 #pragma unroll 1
             for (int c = 0; c < P.n_cols; ++c) {
@@ -1127,17 +1176,25 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
                         using E = decltype(tag);
                         const E* in = (const E*)in_raw;
                         E* out = (E*)out_raw;
-                        if constexpr (decltype(split)::value) {
-                            const uint32_t rows_per = (uint32_t)T / (uint32_t)parts, lo = (uint32_t)h * rows_per;
+                        // a column that arrives in row ranges, or whose base is not aligned to two values, stores each row alone
+                        if (decltype(split)::value || sizeof(E) > 8 || ((uintptr_t)out_raw & (2 * sizeof(E) - 1)) != 0) {
+                            const uint32_t rows_per = decltype(split)::value ? (uint32_t)T / (uint32_t)parts : (uint32_t)T;
+                            const uint32_t lo = decltype(split)::value ? (uint32_t)h * rows_per : 0u;
 #pragma unroll
-                            for (int k = 0; k < K; ++k) {
-                                const uint32_t sr = src[k] - lo;  // source row relative to this range (wraps when below it)
-                                if (orow[k] != SLOT_NONE && sr < rows_per) st_stream(out + orow[k], in[sr]);
+                            for (int k = 0; k < KP; ++k) {
+                                if (orow[k] == SLOT_NONE) continue;
+                                uint32_t sr = (src[k] & 0x7fffu) - lo;  // source row relative to this range (wraps when below it)
+                                if (sr < rows_per) st_stream(out + orow[k], in[sr]);
+                                sr = (src[k] >> 16) - lo;
+                                if ((src[k] & 0x8000u) && sr < rows_per) st_stream(out + orow[k] + 1, in[sr]);
                             }
-                        } else {
+                        } else if constexpr (sizeof(E) <= 8) {
 #pragma unroll
-                            for (int k = 0; k < K; ++k)
-                                if (orow[k] != SLOT_NONE) st_stream(out + orow[k], in[src[k]]);
+                            for (int k = 0; k < KP; ++k) {
+                                if (orow[k] == SLOT_NONE) continue;
+                                if (src[k] & 0x8000u) st_stream_pair(out + orow[k], in[src[k] & 0x7fffu], in[src[k] >> 16]);
+                                else st_stream(out + orow[k], in[src[k] & 0x7fffu]);
+                            }
                         }
                     };
                     onepass_by_width<V, S>(cw, parts, copy_col);

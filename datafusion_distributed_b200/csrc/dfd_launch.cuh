@@ -30,9 +30,13 @@ namespace dfd {
 #define DFD_ONEPASS_SPLIT 1
 #endif
 #ifndef DFD_ONEPASS_MIN_CTAS
-// (a register cap of 72 per thread; with NB = 3 a CTA needs 75.5 KB of shared memory at cfg-2, so 2 of them are resident per SM:
-//  the launch sizes the grid by the occupancy API — see DESIGN.md 4.1 for the sweep)
+// (a register cap of 72 per thread; with NB = 3 a CTA needs 70.5 KB of shared memory at cfg-2, so 3 of them would fit per SM)
 #define DFD_ONEPASS_MIN_CTAS 3
+#endif
+#ifndef DFD_ONEPASS_CTAS_PER_SM
+// persistent grid: at most this many CTAs per SM (fewer if the occupancy API says so).  3 fit at cfg-2 but the store
+// stream of 3 runs slower than that of 2 on H100 (DESIGN.md 4.1)
+#define DFD_ONEPASS_CTAS_PER_SM 2
 #endif
 #ifndef DFD_ONEPASS_K
 #define DFD_ONEPASS_K 10  // rows per consumer thread per tile (tile = 256 x K rows): larger tiles amortise ranking / look-back
@@ -42,11 +46,13 @@ constexpr int FOLLOW_MIN_CTAS = 4;  // follow-up k_scatter launches on the singl
 constexpr int ONEPASS_NB = DFD_ONEPASS_NB;
 constexpr int ONEPASS_SPLIT = DFD_ONEPASS_SPLIT;
 constexpr int ONEPASS_MIN_CTAS = DFD_ONEPASS_MIN_CTAS;
+constexpr int ONEPASS_CTAS_PER_SM = DFD_ONEPASS_CTAS_PER_SM;
 constexpr int TILE_THREADS = DFD_TILE_THREADS;
 constexpr int TILE_K = DFD_TILE_K;
 constexpr int TILE_MIN_CTAS = DFD_TILE_MIN_CTAS;
 // aligned write-out (see k_scatter): used when N <= ALIGNED_MAX_N; each run wastes < 62 virtual slots
 constexpr uint32_t ALIGNED_MAX_N = 16;
+static_assert(ALIGNED_MAX_N == PAIR_ALIGN_MAX_N, "the single-pass local write-out aligns warps for the same N");
 constexpr int TILE_KV = TILE_K + (62 * (int)ALIGNED_MAX_N + TILE_THREADS - 1) / TILE_THREADS;
 constexpr int TILE_ROWS = TILE_THREADS * TILE_K;
 constexpr int ONEPASS_KV = ONEPASS_K + (62 * (int)ALIGNED_MAX_N + TILE_THREADS - 1) / TILE_THREADS;
@@ -81,6 +87,7 @@ static int launch_scatter_kv(const ScatterParams& sp, int sm_count, size_t smem,
                     return cuda_error(e, "cudaFuncSetAttribute(k_scatter_onepass)");
                 if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cfg_per_sm, kern, TILE_THREADS + 32, smem)) != cudaSuccess)
                     return cuda_error(e, "cudaOccupancyMaxActiveBlocksPerMultiprocessor");
+                if (cfg_per_sm > ONEPASS_CTAS_PER_SM) cfg_per_sm = ONEPASS_CTAS_PER_SM;
                 if (cfg_per_sm < 1) cfg_per_sm = 1;
                 cfg_smem = smem;
             }
