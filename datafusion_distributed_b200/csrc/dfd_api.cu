@@ -5,6 +5,7 @@
 // whole-table device passes instead of per-8192-row-batch CPU gathers.
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -52,24 +53,6 @@ int Scratch::ensure(size_t need, int device) {
 }
 
 }  // namespace dfd
-
-int dfd_ctx::drain_events() {
-    if (ev_pending == 0) return DFD_OK;
-    cudaError_t e = cudaEventSynchronize(ev_ring[4 * (ev_pending - 1) + 3]);
-    if (e != cudaSuccess) return dfd::cuda_error(e, "partition kernels");
-    for (size_t i = 0; i < ev_pending; ++i) {
-        cudaEvent_t* ev = &ev_ring[4 * i];
-        float a = 0, b = 0, d = 0;
-        cudaEventElapsedTime(&a, ev[0], ev[1]);
-        cudaEventElapsedTime(&b, ev[1], ev[2]);
-        cudaEventElapsedTime(&d, ev[2], ev[3]);
-        metrics.hist_ms += a;
-        metrics.scan_ms += b;
-        metrics.scatter_ms += d;
-    }
-    ev_pending = 0;
-    return DFD_OK;
-}
 
 using namespace dfd;
 
@@ -122,12 +105,6 @@ static int build_keyset(const dfd_partitioner* p, const dfd_column* cols, int n_
     return DFD_OK;
 }
 
-#define LAUNCH_CHECK(what)                                             \
-    {                                                                  \
-        cudaError_t _e = cudaGetLastError();                           \
-        if (_e != cudaSuccess) return cuda_error(_e, what);            \
-    }
-
 // Aligned write-out gives NVLink peer stores full-size write packets, so it is on for the fused exchange only.
 // A local single-pass launch aligns its stores without it (its KV == K write-out stores warp-aligned output-row
 // pairs, see k_scatter_onepass).  DFD_ALIGNED_WRITEOUT=0/1 forces it.
@@ -137,15 +114,20 @@ bool dfd::use_aligned(uint32_t N, bool peer) {
     return forced >= 0 ? forced == 1 : peer;
 }
 
-// mode: 0 two-pass, 1 single-pass, 2 follow-up of a single-pass launch (see dfd_launch.cuh)
-static int launch_scatter(const ScatterParams& sp, int width, bool fast, bool peer, int mode, int sm_count, size_t smem,
-                          cudaStream_t stream) {
-    if (mode == 1) return peer ? launch_scatter_onepass_peer(sp, width, fast, sm_count, smem, stream)
-                               : launch_scatter_onepass_local(sp, width, fast, sm_count, smem, stream);
-    if (mode == 2) return peer ? launch_scatter_follow_peer(sp, width, fast, sm_count, smem, stream)
-                               : launch_scatter_follow_local(sp, width, fast, sm_count, smem, stream);
-    return peer ? launch_scatter_twopass_peer(sp, width, fast, sm_count, smem, stream)
-                : launch_scatter_twopass_local(sp, width, fast, sm_count, smem, stream);
+template <ScatterKind KIND>
+static int launch_scatter_kind(bool peer, const ScatterParams& sp, int width, bool fast, int sm_count, cudaStream_t stream) {
+    return peer ? launch_scatter_impl<true, KIND>(sp, width, fast, sm_count, stream)
+                : launch_scatter_impl<false, KIND>(sp, width, fast, sm_count, stream);
+}
+
+// One scatter launch of `width` (0: bit columns) through the instantiation of its kind and mode.
+static int launch_scatter(ScatterKind kind, bool peer, const ScatterParams& sp, int width, bool fast, int sm_count, cudaStream_t stream) {
+    switch (kind) {
+        case ScatterKind::TwoPass: return launch_scatter_kind<ScatterKind::TwoPass>(peer, sp, width, fast, sm_count, stream);
+        case ScatterKind::OnePass: return launch_scatter_kind<ScatterKind::OnePass>(peer, sp, width, fast, sm_count, stream);
+        case ScatterKind::FollowUp: return launch_scatter_kind<ScatterKind::FollowUp>(peer, sp, width, fast, sm_count, stream);
+    }
+    return set_error(DFD_ERR_INTERNAL, "unknown scatter kind %d", (int)kind);
 }
 
 // ---- PartitionJob: validation -> K1/K1b -> K2, reusable by the local path and the exchange ----
@@ -256,7 +238,7 @@ int dfd::PartitionJob::prepare(Partitioner* part, const dfd_column* in_cols, int
         d_src = (uint32_t*)((char*)c->var_scratch.ptr + nb);
         d_block_sums = (unsigned long long*)((char*)c->var_scratch.ptr + 2 * nb);
         k_iota_u32<<<(unsigned)(c->sm_count * 8), 256, 0, stream>>>(d_iota, n_rows);
-        LAUNCH_CHECK("k_iota_u32");
+        CUDA_TRY(cudaGetLastError(), "k_iota_u32");
         c->metrics.kernel_launches++;
         PayloadCol ip{};
         ip.in = d_iota;
@@ -287,17 +269,7 @@ int dfd::PartitionJob::prepare(Partitioner* part, const dfd_column* in_cols, int
         c->scratch_done = d_done;
     }
     ev = nullptr;
-    if (c->profiling) {
-        if (c->ev_ring.empty()) {
-            c->ev_ring.resize(4 * dfd_ctx::EV_RING_CALLS);
-            for (auto& e : c->ev_ring) cudaEventCreate(&e);
-        }
-        if (c->ev_pending == dfd_ctx::EV_RING_CALLS) {
-            rc = c->drain_events();
-            if (rc) return rc;
-        }
-        ev = &c->ev_ring[4 * c->ev_pending];
-    }
+    if (c->profiling && (rc = c->phases.next(&ev))) return rc;
     return DFD_OK;
 }
 
@@ -323,69 +295,60 @@ int dfd::PartitionJob::run_hist_scan() {
             switch (nf) { case 1: HIST(false, 1); break; case 2: HIST(false, 2); break; case 4: HIST(false, 4); break; default: HIST(false, 0); }
         }
 #undef HIST
-        LAUNCH_CHECK("k_tile_hist");
+        CUDA_TRY(cudaGetLastError(), "k_tile_hist");
     }
     if (ev) cudaEventRecord(ev[1], stream);
     k_scan_tiles<1024><<<N, 1024, 0, stream>>>(d_hist, d_base, d_totals, p->d_part_starts, d_done, n_tiles, N);
-    LAUNCH_CHECK("k_scan_tiles");
+    CUDA_TRY(cudaGetLastError(), "k_scan_tiles");
     if (ev) cudaEventRecord(ev[2], stream);
     c->metrics.kernel_launches += 2;
     return DFD_OK;
 }
 
-// K2.  dest_base[N]: first output row of each destination (p->d_part_starts in local mode).
-int dfd::PartitionJob::run_scatter(const int64_t* dest_base, void* const* peer_base, int world, uint32_t parts_per_rank,
-                                   const int32_t* abort_flag) {
+// The ScatterParams fields every scatter launch of this job shares.
+int dfd::PartitionJob::scatter_params(ScatterParams& sp, void* const* peer_base, int world, uint32_t parts_per_rank) const {
+    sp = ScatterParams{};
+    sp.keys = ks;
+    sp.st = p->st;
+    sp.mod = p->mod;
+    sp.n_rows = n_rows;
+    sp.n_tiles = n_tiles;
+    sp.N = p->N;
+    sp.parts_per_rank = parts_per_rank ? parts_per_rank : 1;
+    if (peer) {
+        if (world > MAX_RANKS) return set_error(DFD_ERR_UNSUPPORTED, "world size %d > %d", world, MAX_RANKS);
+        for (int r = 0; r < world; ++r) sp.peer_base[r] = peer_base[r];
+    }
+    return DFD_OK;
+}
+
+// One launch per element width (0 = bit columns) in the order 8, 4, 16, 2, 1, 0, each batching at most MAX_COLS_PER_LAUNCH
+// columns of its width; adds the launches to *launches.
+int dfd::PartitionJob::launch_width_groups(ScatterParams& sp, const std::vector<PayloadCol>& cols, ScatterKind kind, int* launches) {
+    static const int kWidths[6] = {8, 4, 16, 2, 1, 0};
+    for (const int width : kWidths) {
+        std::vector<PayloadCol> group;
+        for (const PayloadCol& pc : cols)
+            if (pc.width == width) group.push_back(pc);
+        sp.stage_width = width ? width : 1;
+        for (size_t first = 0; first < group.size(); first += MAX_COLS_PER_LAUNCH) {
+            const size_t n = std::min(group.size() - first, (size_t)MAX_COLS_PER_LAUNCH);
+            std::copy(group.begin() + first, group.begin() + first + n, sp.cols);
+            sp.n_cols = (int32_t)n;
+            int rc = launch_scatter(kind, peer, sp, width, ks.fast_i64 != 0, p->ctx->sm_count, stream);
+            if (rc) return rc;
+            ++*launches;
+        }
+    }
+    return DFD_OK;
+}
+
+// The end of a partition call: its last profiling event and its metrics.
+void dfd::PartitionJob::finish(int launches) {
     Ctx* c = p->ctx;
-    const uint32_t N = p->N;
-    int launches = 0;
-    if (n_rows > 0) {
-        ScatterParams sp{};
-        sp.keys = ks;
-        sp.st = p->st;
-        sp.mod = p->mod;
-        sp.n_rows = n_rows;
-        sp.n_tiles = n_tiles;
-        sp.hist = d_hist;
-        sp.tile_base = d_base;
-        sp.dest_base = dest_base;
-        sp.N = N;
-        sp.parts_per_rank = parts_per_rank ? parts_per_rank : 1;
-        sp.abort_flag = abort_flag;
-        sp.dest_cache = d_dest_cache;
-        if (peer) {
-            if (world > MAX_RANKS) return set_error(DFD_ERR_UNSUPPORTED, "world size %d > %d", world, MAX_RANKS);
-            for (int r = 0; r < world; ++r) sp.peer_base[r] = peer_base[r];
-        }
-        // one launch per element width (0 = bit columns), columns of that width batched
-        static const int kWidths[6] = {8, 4, 16, 2, 1, 0};
-        for (int wi = 0; wi < 6; ++wi) {
-            const int width = kWidths[wi];
-            std::vector<PayloadCol> group;
-            for (const PayloadCol& pc : passes)
-                if (pc.width == width) group.push_back(pc);
-            if (group.empty()) continue;
-            sp.stage_width = width ? width : 1;
-            size_t smem = scatter_smem_bytes<TILE_THREADS, TILE_K>(N, sp.stage_width, peer, use_aligned(N, peer));
-            if (smem > 227 * 1024)
-                return set_error(DFD_ERR_UNSUPPORTED, "num_partitions %u needs %zu B of shared memory per CTA", N, smem);
-            for (size_t first = 0; first < group.size(); first += MAX_COLS_PER_LAUNCH) {
-                size_t n = group.size() - first < (size_t)MAX_COLS_PER_LAUNCH ? group.size() - first : (size_t)MAX_COLS_PER_LAUNCH;
-                for (size_t i = 0; i < n; ++i) sp.cols[i] = group[first + i];
-                sp.n_cols = (int32_t)n;
-                int rc = launch_scatter(sp, width, ks.fast_i64 != 0, peer, 0, c->sm_count, smem, stream);
-                if (rc) return rc;
-                ++launches;
-            }
-        }
-    }
-    if (!var_cols.empty()) {
-        int rc = run_varwidth();
-        if (rc) return rc;
-    }
     if (ev) {
         cudaEventRecord(ev[3], stream);
-        c->ev_pending++;
+        c->phases.commit();
         ev = nullptr;
     }
     c->metrics.kernel_launches += launches;
@@ -394,12 +357,34 @@ int dfd::PartitionJob::run_scatter(const int64_t* dest_base, void* const* peer_b
     c->metrics.rows += (uint64_t)n_rows;
     c->metrics.bytes_in += bytes;
     c->metrics.bytes_out += bytes;
+}
+
+// K2.  dest_base[N]: first output row of each destination (p->d_part_starts in local mode).
+int dfd::PartitionJob::run_scatter(const int64_t* dest_base, void* const* peer_base, int world, uint32_t parts_per_rank,
+                                   const int32_t* abort_flag) {
+    int launches = 0;
+    if (n_rows > 0) {
+        ScatterParams sp;
+        int rc = scatter_params(sp, peer_base, world, parts_per_rank);
+        if (rc) return rc;
+        sp.hist = d_hist;
+        sp.tile_base = d_base;
+        sp.dest_base = dest_base;
+        sp.abort_flag = abort_flag;
+        sp.dest_cache = d_dest_cache;
+        if ((rc = launch_width_groups(sp, passes, ScatterKind::TwoPass, &launches))) return rc;
+    }
+    if (!var_cols.empty()) {
+        int rc = run_varwidth();
+        if (rc) return rc;
+    }
+    finish(launches);
     return DFD_OK;
 }
 
-// Single-pass partition: ONE k_scatter<ONEPASS> launch hashes, ranks, resolves the tile cursors by
-// decoupled look-back and scatters the first width group; further width groups (and bit columns) reuse
-// the per-tile counts / cursors it leaves in d_hist / d_base through the two-pass code path.
+// Single-pass partition: ONE k_scatter_onepass launch hashes, ranks, resolves the tile cursors by decoupled look-back
+// and scatters the first MAX_COLS_PER_LAUNCH fixed-width columns; the other columns follow in k_scatter launches on
+// the same tiling, driven by the per-tile counts / cursors it leaves in d_hist / d_base.
 int dfd::PartitionJob::run_onepass(const OnePassLayout& L) {
     Ctx* c = p->ctx;
     const uint32_t N = p->N;
@@ -422,14 +407,9 @@ int dfd::PartitionJob::run_onepass(const OnePassLayout& L) {
             cudaError_t e = cudaMemsetAsync(c->lb.ptr, 0, c->lb.bytes, stream);
             if (e != cudaSuccess) return cuda_error(e, "cudaMemsetAsync(look-back table)");
         }
-        ScatterParams sp{};
-        sp.keys = ks;
-        sp.st = p->st;
-        sp.mod = p->mod;
-        sp.n_rows = n_rows;
-        sp.n_tiles = n_tiles;
-        sp.N = N;
-        sp.parts_per_rank = L.parts_per_rank ? L.parts_per_rank : 1;
+        ScatterParams sp;
+        int rc = scatter_params(sp, L.peer_base, L.world, L.parts_per_rank);
+        if (rc) return rc;
         sp.dest_base = L.d_dest_base;
         sp.dest_cap = L.d_dest_cap;
         sp.region_stride = L.region_stride;
@@ -442,13 +422,9 @@ int dfd::PartitionJob::run_onepass(const OnePassLayout& L) {
         sp.overflow_out = L.d_overflow;
         sp.ready_flags = L.ready_flags;
         sp.ready_epoch = L.ready_epoch;
-        if (peer) {
-            if (L.world > MAX_RANKS) return set_error(DFD_ERR_UNSUPPORTED, "world size %d > %d", L.world, MAX_RANKS);
-            for (int r = 0; r < L.world; ++r) sp.peer_base[r] = L.peer_base[r];
-        }
-        // ONE single-pass launch moves every fixed-width column (any mix of widths up to the widest, per-column element type
-        // inside the kernel): the rows are hashed and ranked once.  Bit columns (validity / booleans) and columns beyond the
-        // per-launch limit follow through k_scatter on the same tiling, driven by the counts / cursors the first launch leaves.
+        // ONE single-pass launch moves the first MAX_COLS_PER_LAUNCH fixed-width columns (any mix of widths up to the
+        // widest, per-column element type inside the kernel): the rows are hashed and ranked once.  Bit columns (validity /
+        // booleans) and the fixed-width columns past the per-launch limit are the follow-ups.
         std::vector<PayloadCol> fixed, rest;
         int maxw = 0;
         for (const PayloadCol& pc : passes) {
@@ -456,72 +432,42 @@ int dfd::PartitionJob::run_onepass(const OnePassLayout& L) {
             else rest.push_back(pc);
         }
         if (fixed.empty()) return set_error(DFD_ERR_INTERNAL, "single-pass mode needs a fixed-width column");
-        {
-            for (size_t i = 0; i < fixed.size(); ++i) sp.cols[i] = fixed[i];
-            sp.n_cols = (int32_t)fixed.size();
-            sp.stage_width = maxw;
-            sp.hist_out = rest.empty() ? nullptr : d_hist;
-            sp.base_out = rest.empty() ? nullptr : d_base;
-            // the ring's element type is at most 8 bytes: 16-byte columns travel as two row-range items per tile (see the kernel),
-            // which keeps the slots at tile x 8 bytes and the CTA count per SM independent of the schema
-            const int ring_w = maxw > 8 ? 8 : maxw;
-            int rc = launch_scatter(sp, ring_w, ks.fast_i64 != 0 && ring_w >= 8, peer, 1, c->sm_count, 0, stream);
-            if (rc) return rc;
-            ++launches;
-            // the follow-up launches take the two-pass code path over the counts / cursors just written
-            sp.hist = d_hist;
-            sp.tile_base = d_base;
-            sp.abort_flag = L.d_overflow;
-        }
-        static const int kWidths[6] = {8, 4, 16, 2, 1, 0};
-        for (int wi = 0; wi < 6 && !rest.empty(); ++wi) {
-            const int width = kWidths[wi];
-            std::vector<PayloadCol> group;
-            for (const PayloadCol& pc : rest)
-                if (pc.width == width) group.push_back(pc);
-            if (group.empty()) continue;
-            sp.stage_width = width ? width : 1;
-            for (size_t f0 = 0; f0 < group.size(); f0 += MAX_COLS_PER_LAUNCH) {
-                size_t n = group.size() - f0 < (size_t)MAX_COLS_PER_LAUNCH ? group.size() - f0 : (size_t)MAX_COLS_PER_LAUNCH;
-                for (size_t i = 0; i < n; ++i) sp.cols[i] = group[f0 + i];
-                sp.n_cols = (int32_t)n;
-                int rc = launch_scatter(sp, width, ks.fast_i64 != 0, peer, 2, c->sm_count, 0, stream);
-                if (rc) return rc;
-                ++launches;
-            }
-        }
+        std::copy(fixed.begin(), fixed.end(), sp.cols);
+        sp.n_cols = (int32_t)fixed.size();
+        sp.stage_width = maxw;
+        sp.hist_out = rest.empty() ? nullptr : d_hist;
+        sp.base_out = rest.empty() ? nullptr : d_base;
+        // the ring's element type is at most 8 bytes: 16-byte columns travel as two row-range items per tile (see the kernel),
+        // which keeps the slots at tile x 8 bytes and the CTA count per SM independent of the schema
+        const int ring_w = maxw > 8 ? 8 : maxw;
+        if ((rc = launch_scatter(ScatterKind::OnePass, peer, sp, ring_w, ks.fast_i64 != 0 && ring_w >= 8, c->sm_count, stream))) return rc;
+        ++launches;
+        // the follow-up launches read the counts / cursors just written
+        sp.hist = d_hist;
+        sp.tile_base = d_base;
+        sp.abort_flag = L.d_overflow;
+        if ((rc = launch_width_groups(sp, rest, ScatterKind::FollowUp, &launches))) return rc;
     }
-    if (ev) {
-        cudaEventRecord(ev[3], stream);
-        c->ev_pending++;
-        ev = nullptr;
-    }
-    c->metrics.kernel_launches += launches;
-    c->metrics.scatter_launches += launches;
-    c->metrics.calls++;
-    c->metrics.rows += (uint64_t)n_rows;
-    c->metrics.bytes_in += bytes;
-    c->metrics.bytes_out += bytes;
+    finish(launches);
     return DFD_OK;
 }
 
 template <typename OFF>
 static int launch_varwidth(const dfd::PartitionJob::VarCol& vc, const uint32_t* d_src, unsigned long long* d_block_sums,
-                           int64_t n_rows, int sm_count, cudaStream_t stream) {
+                           int64_t n_rows, cudaStream_t stream) {
     const int64_t n_blocks = (n_rows + VAR_BLOCK * VAR_ITEMS - 1) / (VAR_BLOCK * VAR_ITEMS);
     const OFF* in_off = (const OFF*)vc.in.offsets;
     OFF* out_off = (OFF*)vc.out.offsets;
     k_var_block_sums<OFF><<<(unsigned)n_blocks, VAR_BLOCK, 0, stream>>>(in_off, vc.in.offset, d_src, n_rows, d_block_sums);
-    LAUNCH_CHECK("k_var_block_sums");
+    CUDA_TRY(cudaGetLastError(), "k_var_block_sums");
     k_var_scan_block_sums<<<1, 1024, 0, stream>>>(d_block_sums, n_blocks);
-    LAUNCH_CHECK("k_var_scan_block_sums");
+    CUDA_TRY(cudaGetLastError(), "k_var_scan_block_sums");
     k_var_write_offsets<OFF><<<(unsigned)n_blocks, VAR_BLOCK, 0, stream>>>(in_off, vc.in.offset, d_src, n_rows, d_block_sums, out_off);
-    LAUNCH_CHECK("k_var_write_offsets");
+    CUDA_TRY(cudaGetLastError(), "k_var_write_offsets");
     const int64_t copy_blocks = (n_rows + 255) / 256;
-    (void)sm_count;
     k_var_copy_bytes<OFF><<<(unsigned)(copy_blocks > 0x7fffffffLL ? 0x7fffffffLL : copy_blocks), 256, 0, stream>>>(in_off, vc.in.offset, (const uint8_t*)vc.in.values, d_src, out_off,
                                                                        (uint8_t*)vc.out.values, n_rows);
-    LAUNCH_CHECK("k_var_copy_bytes");
+    CUDA_TRY(cudaGetLastError(), "k_var_copy_bytes");
     return DFD_OK;
 }
 
@@ -534,8 +480,8 @@ int dfd::PartitionJob::run_varwidth() {
             if (e != cudaSuccess) return cuda_error(e, "cudaMemsetAsync");
             continue;
         }
-        int rc = vc.in.kind == DFD_COL_LARGE_UTF8 ? launch_varwidth<int64_t>(vc, d_src, d_block_sums, n_rows, c->sm_count, stream)
-                                                  : launch_varwidth<int32_t>(vc, d_src, d_block_sums, n_rows, c->sm_count, stream);
+        int rc = vc.in.kind == DFD_COL_LARGE_UTF8 ? launch_varwidth<int64_t>(vc, d_src, d_block_sums, n_rows, stream)
+                                                  : launch_varwidth<int32_t>(vc, d_src, d_block_sums, n_rows, stream);
         if (rc) return rc;
         c->metrics.kernel_launches += 4;
     }
@@ -545,14 +491,14 @@ int dfd::PartitionJob::run_varwidth() {
 int dfd::launch_bits_to_bytes(const uint8_t* bits, int64_t bit_offset, int64_t n, uint8_t* out, cudaStream_t s) {
     if (n <= 0) return DFD_OK;
     k_bits_to_bytes<<<(unsigned)((n + 255) / 256 > 4096 ? 4096 : (n + 255) / 256), 256, 0, s>>>(bits, bit_offset, n, out);
-    LAUNCH_CHECK("k_bits_to_bytes");
+    CUDA_TRY(cudaGetLastError(), "k_bits_to_bytes");
     return DFD_OK;
 }
 
 int dfd::launch_bytes_to_bits(const uint8_t* in, int64_t n, void* out_words, cudaStream_t s) {
     if (n <= 0) return DFD_OK;
     k_bytes_to_bits<<<(unsigned)((n + 255) / 256 > 4096 ? 4096 : (n + 255) / 256), 256, 0, s>>>(in, n, (unsigned*)out_words);
-    LAUNCH_CHECK("k_bytes_to_bits");
+    CUDA_TRY(cudaGetLastError(), "k_bytes_to_bits");
     return DFD_OK;
 }
 
@@ -561,7 +507,7 @@ int dfd::launch_offsets_to_lengths(const void* off, int ow, int64_t n, void* len
     const unsigned grid = (unsigned)((n + 255) / 256 > 4096 ? 4096 : (n + 255) / 256);
     if (ow == 8) k_offsets_to_lengths<int64_t><<<grid, 256, 0, s>>>((const int64_t*)off, n, (int64_t*)len);
     else k_offsets_to_lengths<int32_t><<<grid, 256, 0, s>>>((const int32_t*)off, n, (int32_t*)len);
-    LAUNCH_CHECK("k_offsets_to_lengths");
+    CUDA_TRY(cudaGetLastError(), "k_offsets_to_lengths");
     return DFD_OK;
 }
 
@@ -569,7 +515,7 @@ int dfd::launch_var_dest_bytes(const void* off, int ow, const int64_t* part_star
     const unsigned grid = (N + 255) / 256;
     if (ow == 8) k_var_dest_bytes<int64_t><<<grid, 256, 0, s>>>((const int64_t*)off, part_starts, N, bytes, first);
     else k_var_dest_bytes<int32_t><<<grid, 256, 0, s>>>((const int32_t*)off, part_starts, N, bytes, first);
-    LAUNCH_CHECK("k_var_dest_bytes");
+    CUDA_TRY(cudaGetLastError(), "k_var_dest_bytes");
     return DFD_OK;
 }
 
@@ -581,13 +527,22 @@ int dfd::launch_lengths_to_offsets(const void* len, int ow, int64_t n, unsigned 
     const int64_t n_blocks = (n + VAR_BLOCK * VAR_ITEMS - 1) / (VAR_BLOCK * VAR_ITEMS);
     if (ow == 8) k_len_block_sums<int64_t><<<(unsigned)n_blocks, VAR_BLOCK, 0, s>>>((const int64_t*)len, n, block_sums);
     else k_len_block_sums<int32_t><<<(unsigned)n_blocks, VAR_BLOCK, 0, s>>>((const int32_t*)len, n, block_sums);
-    LAUNCH_CHECK("k_len_block_sums");
+    CUDA_TRY(cudaGetLastError(), "k_len_block_sums");
     k_var_scan_block_sums<<<1, 1024, 0, s>>>(block_sums, n_blocks);
-    LAUNCH_CHECK("k_var_scan_block_sums");
+    CUDA_TRY(cudaGetLastError(), "k_var_scan_block_sums");
     if (ow == 8) k_len_write_offsets<int64_t><<<(unsigned)n_blocks, VAR_BLOCK, 0, s>>>((const int64_t*)len, n, block_sums, (int64_t*)out_off);
     else k_len_write_offsets<int32_t><<<(unsigned)n_blocks, VAR_BLOCK, 0, s>>>((const int32_t*)len, n, block_sums, (int32_t*)out_off);
-    LAUNCH_CHECK("k_len_write_offsets");
+    CUDA_TRY(cudaGetLastError(), "k_len_write_offsets");
     return DFD_OK;
+}
+
+// ahash RandomState::with_seeds: seed ^ PI2 (random_state.rs); seeds NULL = (0, 0, 0, 0), DataFusion's
+// REPARTITION_RANDOM_STATE.
+static HashState hash_state_from_seeds(const uint64_t* seeds) {
+    static const uint64_t PI2[4] = {0x452821e638d01377ULL, 0xbe5466cf34e90c6cULL, 0xc0ac29b7c97c50ddULL, 0x3f84d5b5b5470917ULL};
+    uint64_t s[4] = {0, 0, 0, 0};
+    if (seeds) memcpy(s, seeds, sizeof s);
+    return HashState{s[0] ^ PI2[0], s[1] ^ PI2[1], s[2] ^ PI2[2], s[3] ^ PI2[3]};
 }
 
 int dfd::partition_device_locked(Partitioner* p, const dfd_column* in_cols, int n_cols, int64_t n_rows,
@@ -618,10 +573,7 @@ int dfd::hash_columns_locked(Ctx* c, const dfd_column* in_cols, int n_cols, int6
         }
     }
     tmp.key_dicts.assign((size_t)n_cols, dfd_partitioner::KeyDict{});
-    static const uint64_t PI2[4] = {0x452821e638d01377ULL, 0xbe5466cf34e90c6cULL, 0xc0ac29b7c97c50ddULL, 0x3f84d5b5b5470917ULL};
-    uint64_t sd[4] = {0, 0, 0, 0};
-    if (seeds) memcpy(sd, seeds, sizeof sd);
-    tmp.st = HashState{sd[0] ^ PI2[0], sd[1] ^ PI2[1], sd[2] ^ PI2[2], sd[3] ^ PI2[3]};
+    tmp.st = hash_state_from_seeds(seeds);
     if (n_rows == 0) return DFD_OK;
     KeySet ks;
     int rc = build_keyset(&tmp, cols, n_cols, &ks);
@@ -629,7 +581,7 @@ int dfd::hash_columns_locked(Ctx* c, const dfd_column* in_cols, int n_cols, int6
     int64_t blocks = (n_rows + 255) / 256;
     if (blocks > (int64_t)c->sm_count * 32) blocks = (int64_t)c->sm_count * 32;
     k_row_hashes<<<(unsigned)blocks, 256, 0, stream>>>(ks, tmp.st, n_rows, hashes_device);
-    LAUNCH_CHECK("k_row_hashes");
+    CUDA_TRY(cudaGetLastError(), "k_row_hashes");
     c->metrics.kernel_launches++;
     return DFD_OK;
 }
@@ -702,7 +654,6 @@ void dfd_ctx_destroy(dfd_ctx* c) {
     if (c->flush.ptr) cudaFree(c->flush.ptr);
     if (c->var_scratch.ptr) cudaFree(c->var_scratch.ptr);
     if (c->lb.ptr) cudaFree(c->lb.ptr);
-    for (auto& ev : c->ev_ring) cudaEventDestroy(ev);
     cudaEventDestroy(c->timer_a);
     cudaEventDestroy(c->timer_b);
     cudaStreamDestroy(c->stream);
@@ -807,15 +758,19 @@ int dfd_timer_stop(dfd_ctx* c, float* out_ms) {
 int dfd_metrics_get(dfd_ctx* c, dfd_metrics* out) {
     CTX_GUARD(c);
     if (!out) return set_error(DFD_ERR_INVALID_ARGUMENT, "out is NULL");
-    int rc = c->drain_events();
+    int rc = c->phases.drain();
     if (rc) return rc;
     *out = c->metrics;
+    out->hist_ms = c->phases.sum_ms[0];
+    out->scan_ms = c->phases.sum_ms[1];
+    out->scatter_ms = c->phases.sum_ms[2];
     return DFD_OK;
 }
 
 int dfd_metrics_reset(dfd_ctx* c) {
     CTX_GUARD(c);
-    c->drain_events();
+    c->phases.drain();
+    c->phases.reset();
     memset(&c->metrics, 0, sizeof c->metrics);
     return DFD_OK;
 }
@@ -843,13 +798,7 @@ int dfd_partitioner_create(dfd_ctx* c, uint32_t num_partitions, const int32_t* k
     p->key_cols.assign(key_cols, key_cols + n_keys);
     p->key_modes.assign((size_t)n_keys, DFD_KEY_HASH_PLAIN);
     p->key_dicts.assign((size_t)n_keys, dfd_partitioner::KeyDict{});
-    // ahash RandomState::with_seeds: seed ^ PI2 (random_state.rs); DataFusion's
-    // REPARTITION_RANDOM_STATE uses seeds (0,0,0,0).
-    static const uint64_t PI2[4] = {0x452821e638d01377ULL, 0xbe5466cf34e90c6cULL, 0xc0ac29b7c97c50ddULL,
-                                    0x3f84d5b5b5470917ULL};
-    uint64_t s[4] = {0, 0, 0, 0};
-    if (seeds) memcpy(s, seeds, sizeof s);
-    p->st = HashState{s[0] ^ PI2[0], s[1] ^ PI2[1], s[2] ^ PI2[2], s[3] ^ PI2[3]};
+    p->st = hash_state_from_seeds(seeds);
     p->mod = make_modn(num_partitions);
     {
         CTX_GUARD(c);
@@ -932,7 +881,7 @@ int dfd_partition_ids_device(dfd_partitioner* p, const dfd_column* cols, int n_c
     int64_t cap = (int64_t)c->sm_count * 32;
     if (blocks > cap) blocks = cap;
     k_partition_ids<<<(unsigned)blocks, 256, 0, c->stream>>>(ks, p->st, p->mod, n_rows, dest_device);
-    LAUNCH_CHECK("k_partition_ids");
+    CUDA_TRY(cudaGetLastError(), "k_partition_ids");
     c->metrics.kernel_launches++;
     cudaError_t e = cudaStreamSynchronize(c->stream);
     return e == cudaSuccess ? DFD_OK : cuda_error(e, "k_partition_ids");

@@ -100,11 +100,6 @@ int nccl_error(ncclResult_t r, const char* what) {
         ncclResult_t _r = (call);                              \
         if (_r != ncclSuccess) return nccl_error(_r, what);    \
     }
-#define CUDA_TRY(call, what)                                   \
-    {                                                          \
-        cudaError_t _e = (call);                               \
-        if (_e != cudaSuccess) return cuda_error(_e, what);    \
-    }
 
 // dest_base / part_starts / overflow check on the device (fused mode), from the
 // all-gathered count matrix counts[T][N]: no host round trip before K2.
@@ -348,11 +343,7 @@ struct dfd_exchange {
     void* h_runs = nullptr;                 // pinned staging of the same
     size_t runs_cap = 0;
     uint64_t push_shuffles = 0;
-    // phase timing of the single-pass shuffle (profiling mode): 4 events per shuffle, drained by dfd_exchange_phase_ms
-    std::vector<cudaEvent_t> pev;
-    size_t pev_pending = 0;
-    double phase_ms[3] = {0, 0, 0};
-    uint64_t phase_shuffles = 0;
+    EventRing phases;  // profiling: the three stream phases of every single-pass shuffle (dfd_exchange_phase_ms)
     uint64_t onepass_fallbacks = 0;
     // What dfd_exchange_collect / _wait / _pending_segments report on: the last shuffle, if it left a result to pick up.
     // Every shuffle entry point resets it to NONE first and sets its own kind only on success.
@@ -480,7 +471,6 @@ void dfd_exchange_destroy(dfd_exchange* x) {
         if (x->comm) nccl_api()->CommDestroy(x->comm);
         cudaFree(x->window);
         cudaFree(x->d_peer_hdr);
-        for (auto& e : x->pev) cudaEventDestroy(e);
         cudaFree(x->d_flags);
         cudaFree(x->d_meta);
         cudaFree(x->d_runs);
@@ -723,25 +713,11 @@ static int onepass_shuffle_locked(dfd_exchange* x, dfd_partitioner* part, const 
     if (sub_cap < 32) return set_error(DFD_ERR_CAPACITY, "receive window (%zu B) too small for %u x %d sub-windows", x->window_bytes, P, T);
     const unsigned long long epoch = ++x->epoch;
     ExchangeHeader* hdr = (ExchangeHeader*)x->window;
+    int rc;
     cudaEvent_t* pe = nullptr;
     if (c->profiling) {
-        constexpr size_t RING = 64;
-        if (x->pev.empty()) {
-            x->pev.resize(4 * RING);
-            for (auto& e : x->pev) cudaEventCreate(&e);
-        }
-        if (x->pev_pending == RING) {  // drain
-            cudaEventSynchronize(x->pev[4 * RING - 1]);
-            for (size_t i = 0; i < RING; ++i)
-                for (int k = 0; k < 3; ++k) {
-                    float ms = 0;
-                    cudaEventElapsedTime(&ms, x->pev[4 * i + k], x->pev[4 * i + k + 1]);
-                    x->phase_ms[k] += ms;
-                }
-            x->phase_shuffles += RING;
-            x->pev_pending = 0;
-        }
-        pe = &x->pev[4 * x->pev_pending++];
+        if ((rc = x->phases.next(&pe))) return rc;
+        x->phases.commit();
         cudaEventRecord(pe[0], s);
     }
     // consumer half: my window is free (everything enqueued on my stream so far — i.e. my reads of the previous shuffle — is ordered before)
@@ -749,7 +725,6 @@ static int onepass_shuffle_locked(dfd_exchange* x, dfd_partitioner* part, const 
     if (pe) cudaEventRecord(pe[1], s);
     CUDA_TRY(cudaGetLastError(), "k_xchg_signal_ready");
     CUDA_TRY(cudaMemsetAsync(x->d_flags, 0, 8, s), "memset flags");
-    int rc;
     PartitionJob job;
     job.onepass_tiling = true;
     if ((rc = job.prepare(part, in_cols, n_cols, n_rows, outs.data(), true, s))) return rc;
@@ -1678,18 +1653,11 @@ int dfd_exchange_phase_ms(dfd_exchange* x, double* out3, uint64_t* n_shuffles) {
     std::lock_guard<std::mutex> lk(c->mu);
     CUDA_TRY(cudaSetDevice(c->device), "cudaSetDevice");
     CUDA_TRY(cudaStreamSynchronize(c->stream), "sync");
-    for (size_t i = 0; i < x->pev_pending; ++i)
-        for (int k = 0; k < 3; ++k) {
-            float ms = 0;
-            cudaEventElapsedTime(&ms, x->pev[4 * i + k], x->pev[4 * i + k + 1]);
-            x->phase_ms[k] += ms;
-        }
-    x->phase_shuffles += x->pev_pending;
-    x->pev_pending = 0;
-    for (int k = 0; k < 3; ++k) out3[k] = x->phase_shuffles ? x->phase_ms[k] / (double)x->phase_shuffles : 0.0;
-    if (n_shuffles) *n_shuffles = x->phase_shuffles;
-    x->phase_ms[0] = x->phase_ms[1] = x->phase_ms[2] = 0;
-    x->phase_shuffles = 0;
+    EventRing& r = x->phases;
+    if (int rc = r.drain()) return rc;
+    for (int k = 0; k < 3; ++k) out3[k] = r.calls ? r.sum_ms[k] / (double)r.calls : 0.0;
+    if (n_shuffles) *n_shuffles = r.calls;
+    r.reset();
     return DFD_OK;
 }
 

@@ -17,10 +17,65 @@ namespace dfd {
 int set_error(int code, const char* fmt, ...);
 int cuda_error(cudaError_t e, const char* what);
 
+#define CUDA_TRY(call, what)                                   \
+    {                                                          \
+        cudaError_t _e = (call);                               \
+        if (_e != cudaSuccess) return dfd::cuda_error(_e, what); \
+    }
+
 struct Scratch {
     void* ptr = nullptr;
     size_t bytes = 0;
     int ensure(size_t need, int device);
+};
+
+// Profiling: the CUDA events of up to CALLS calls, four per call (three consecutive phases), recorded without a sync.
+// The phase durations are summed when the ring is full and whenever the owner reads them.  (Inline: the exchange is
+// also linked without dfd_api.cu.)
+struct EventRing {
+    static constexpr size_t CALLS = 64;
+    std::vector<cudaEvent_t> ev;     // 4 per call, created on first use
+    size_t pending = 0;              // calls recorded, not yet summed
+    double sum_ms[3] = {0, 0, 0};    // phase durations of the calls summed since reset()
+    uint64_t calls = 0;              // ... and their number
+
+    EventRing() = default;
+    EventRing(const EventRing&) = delete;
+    EventRing& operator=(const EventRing&) = delete;
+    ~EventRing() {
+        for (cudaEvent_t e : ev) cudaEventDestroy(e);
+    }
+    // The event quad of the next call (summing the ring first if it is full); commit() once its last event is recorded.
+    int next(cudaEvent_t** quad) {
+        if (ev.empty()) {
+            ev.resize(4 * CALLS);
+            for (cudaEvent_t& e : ev) cudaEventCreate(&e);
+        }
+        if (pending == CALLS) {
+            if (int rc = drain()) return rc;
+        }
+        *quad = &ev[4 * pending];
+        return DFD_OK;
+    }
+    void commit() { ++pending; }
+    // Waits for the recorded calls and adds their phase durations to the sums.
+    int drain() {
+        if (pending == 0) return DFD_OK;
+        CUDA_TRY(cudaEventSynchronize(ev[4 * pending - 1]), "partition kernels");
+        for (size_t i = 0; i < pending; ++i)
+            for (int k = 0; k < 3; ++k) {
+                float ms = 0;
+                cudaEventElapsedTime(&ms, ev[4 * i + k], ev[4 * i + k + 1]);
+                sum_ms[k] += ms;
+            }
+        calls += pending;
+        pending = 0;
+        return DFD_OK;
+    }
+    void reset() {
+        sum_ms[0] = sum_ms[1] = sum_ms[2] = 0;
+        calls = 0;
+    }
 };
 
 }  // namespace dfd
@@ -31,11 +86,7 @@ struct dfd_ctx {
     int sm_count = 132;
     size_t l2_bytes = 0;
     cudaStream_t stream = nullptr;  // compute stream: K1/K1b/K2 launch here
-    // profiling: ring of event quads recorded without syncing; drained lazily
-    std::vector<cudaEvent_t> ev_ring;  // 4 events per call
-    size_t ev_pending = 0;             // calls recorded, not yet accumulated
-    static constexpr size_t EV_RING_CALLS = 64;
-    int drain_events();                // sync + accumulate into metrics
+    dfd::EventRing phases;          // profiling: K1 / K1b / K2 phases of every partition call (dfd_metrics hist/scan/scatter_ms)
     cudaEvent_t timer_a = nullptr, timer_b = nullptr;
     bool profiling = false;
     dfd::Scratch scratch;  // tile histograms / cursors
@@ -60,7 +111,6 @@ struct dfd_partitioner {
     dfd::HashState st{};
     dfd::ModN mod{};
     int64_t* d_part_starts = nullptr;  // [N+1]
-    size_t smem_configured = 0;
     // single-pass (region layout) state: results of the last dfd_partition_device_onepass
     int64_t* d_counts = nullptr;       // [N] rows per destination | [N] dest_base | [N] dest_cap (exact re-run) | overflow flag
     int64_t* h_pin = nullptr;          // pinned: [N] counts, then the overflow flag
@@ -72,6 +122,11 @@ struct dfd_partitioner {
 namespace dfd {
 using Ctx = ::dfd_ctx;
 using Partitioner = ::dfd_partitioner;
+
+// What a scatter launch is: the two-pass k_scatter on the K1 tiling (TILE_K), the single-pass k_scatter_onepass
+// (ONEPASS_K), or a follow-up k_scatter on the single-pass tiling: further width groups / bit columns of a single-pass
+// call, driven by the per-tile counts and cursors the single-pass launch left in hist_out / base_out.
+enum class ScatterKind { TwoPass, OnePass, FollowUp };
 
 // One partition call split into its stages so the exchange can put the count
 // all-gather between K1b and K2.  Caller holds ctx->mu and has set the device.
@@ -116,6 +171,11 @@ struct PartitionJob {
         unsigned long long ready_epoch = 0;
     };
     int run_onepass(const OnePassLayout& L);
+
+  private:
+    int scatter_params(ScatterParams& sp, void* const* peer_base, int world, uint32_t parts_per_rank) const;
+    int launch_width_groups(ScatterParams& sp, const std::vector<PayloadCol>& cols, ScatterKind kind, int* launches);
+    void finish(int launches);
 };
 
 constexpr uint32_t ONEPASS_MAX_N = 256;  // above this the per-tile look-back costs more than the K1 pass it replaces
@@ -173,13 +233,16 @@ __attribute__((weak)) int launch_stage_sizes(const StageSize* jobs, int n_jobs, 
 
 // Aligned write-out (k_scatter KV > K) is used for the peer-store exchange at small N (full-size NVLink write packets).
 bool use_aligned(uint32_t N, bool peer);
-// Kernel launch dispatch, one translation unit each (dfd_scatter_*.cu, templates in dfd_launch.cuh)
-int launch_scatter_twopass_local(const ScatterParams& sp, int width, bool fast, int sm_count, size_t smem, cudaStream_t stream);
-int launch_scatter_twopass_peer(const ScatterParams& sp, int width, bool fast, int sm_count, size_t smem, cudaStream_t stream);
-int launch_scatter_onepass_local(const ScatterParams& sp, int width, bool fast, int sm_count, size_t smem, cudaStream_t stream);
-int launch_scatter_onepass_peer(const ScatterParams& sp, int width, bool fast, int sm_count, size_t smem, cudaStream_t stream);
-int launch_scatter_follow_local(const ScatterParams& sp, int width, bool fast, int sm_count, size_t smem, cudaStream_t stream);
-int launch_scatter_follow_peer(const ScatterParams& sp, int width, bool fast, int sm_count, size_t smem, cudaStream_t stream);
+// One scatter launch of a width group (template in dfd_launch.cuh).  Each (PEER, KIND) is instantiated in a translation unit
+// of its own (dfd_scatter_<kind>_<local|peer>.cu) so that they compile in parallel; nowhere else.
+template <bool PEER, ScatterKind KIND>
+int launch_scatter_impl(const ScatterParams& sp, int width, bool fast, int sm_count, cudaStream_t stream);
+extern template int launch_scatter_impl<false, ScatterKind::TwoPass>(const ScatterParams&, int, bool, int, cudaStream_t);
+extern template int launch_scatter_impl<true, ScatterKind::TwoPass>(const ScatterParams&, int, bool, int, cudaStream_t);
+extern template int launch_scatter_impl<false, ScatterKind::OnePass>(const ScatterParams&, int, bool, int, cudaStream_t);
+extern template int launch_scatter_impl<true, ScatterKind::OnePass>(const ScatterParams&, int, bool, int, cudaStream_t);
+extern template int launch_scatter_impl<false, ScatterKind::FollowUp>(const ScatterParams&, int, bool, int, cudaStream_t);
+extern template int launch_scatter_impl<true, ScatterKind::FollowUp>(const ScatterParams&, int, bool, int, cudaStream_t);
 
 // Column kinds that only the host operator hands to hash_columns_locked, never part of the C ABI: Interval(DayTime) (8 bytes)
 // and Interval(MonthDayNano) (16 bytes) dictionary VALUES, hashed field by field like interval keys (KEY_HASH_INTERVAL_*).

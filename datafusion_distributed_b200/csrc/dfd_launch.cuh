@@ -1,6 +1,8 @@
 // dfd_launch.cuh — tile geometry and the template dispatch of the scatter kernels.
-// The instantiations are spread over several translation units (dfd_scatter_*.cu) so that they compile in
-// parallel; dfd_api.cu only sees the declarations at the bottom of dfd_internal.h.
+// launch_scatter_impl<PEER, KIND> is explicitly instantiated once per (PEER, KIND), each in a translation unit of its own
+// (dfd_scatter_<kind>_<local|peer>.cu), so that the kernels compile in parallel.  Everywhere else the extern template
+// declarations in dfd_internal.h keep the compiler from instantiating it again: dfd_api.cu includes this header for the
+// tile geometry only.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -59,13 +61,12 @@ constexpr int ONEPASS_KV = ONEPASS_K + (62 * (int)ALIGNED_MAX_N + TILE_THREADS -
 constexpr int ONEPASS_ROWS = TILE_THREADS * ONEPASS_K;
 
 
-// MODE: 0 = two-pass k_scatter on the K1 tiling (TILE_K); 1 = single-pass k_scatter_onepass (ONEPASS_K);
-//       2 = "follow-up" k_scatter on the SINGLE-PASS tiling: further column-width groups / bit columns of a single-pass
-//           call, driven by the per-tile counts and cursors the single-pass launch left in hist_out / base_out
-template <bool FAST, typename V, bool PEER, bool ALIGNED, int MODE>
-static int launch_scatter_kv(const ScatterParams& sp, int sm_count, size_t smem, cudaStream_t stream) {
+// KIND picks the kernel and its tiling (see ScatterKind), V the element type, ALIGNED the write-out.  The dynamic shared
+// memory of every kind is sized and checked here.
+template <bool FAST, typename V, bool PEER, bool ALIGNED, ScatterKind KIND>
+static int launch_scatter_kv(const ScatterParams& sp, int sm_count, cudaStream_t stream) {
     cudaError_t e;
-    if constexpr (MODE == 1) {
+    if constexpr (KIND == ScatterKind::OnePass) {
         // run_onepass launches a ring of min(widest column, 8) bytes and takes the fast key path only with an 8-byte ring:
         // the other single-pass instantiations are never launched, so they are not compiled
         if constexpr (std::is_same<V, BitColumn>::value) {
@@ -77,7 +78,7 @@ static int launch_scatter_kv(const ScatterParams& sp, int sm_count, size_t smem,
         } else {
             constexpr int KV = ALIGNED ? ONEPASS_KV : ONEPASS_K;
             auto kern = k_scatter_onepass<TILE_THREADS, ONEPASS_K, KV, ONEPASS_NB, ONEPASS_SPLIT, ONEPASS_MIN_CTAS, FAST, V, PEER>;
-            smem = onepass_smem_bytes<TILE_THREADS, ONEPASS_K, ONEPASS_NB, ONEPASS_SPLIT>(sp.N, (int)sizeof(V), PEER, ALIGNED);
+            const size_t smem = onepass_smem_bytes<TILE_THREADS, ONEPASS_K, ONEPASS_NB, ONEPASS_SPLIT>(sp.N, (int)sizeof(V), PEER, ALIGNED);
             if (smem > 227 * 1024) return set_error(DFD_ERR_UNSUPPORTED, "single-pass kernel needs %zu B of shared memory per CTA", smem);
             // (static per instantiation: the attribute and the occupancy are properties of the kernel + smem size)
             static thread_local size_t cfg_smem = 0;
@@ -96,12 +97,14 @@ static int launch_scatter_kv(const ScatterParams& sp, int sm_count, size_t smem,
             kern<<<(unsigned)grid, TILE_THREADS + 32, smem, stream>>>(sp);
         }
     } else {
-        constexpr int K = MODE == 2 ? ONEPASS_K : TILE_K;
-        constexpr int KV = ALIGNED ? (MODE == 2 ? ONEPASS_KV : TILE_KV) : K;
-        constexpr int CTAS = MODE == 2 ? FOLLOW_MIN_CTAS : TILE_MIN_CTAS;
+        constexpr bool FOLLOW = KIND == ScatterKind::FollowUp;
+        constexpr int K = FOLLOW ? ONEPASS_K : TILE_K;
+        constexpr int KV = ALIGNED ? (FOLLOW ? ONEPASS_KV : TILE_KV) : K;
+        constexpr int CTAS = FOLLOW ? FOLLOW_MIN_CTAS : TILE_MIN_CTAS;
         auto kern = k_scatter<TILE_THREADS, K, KV, CTAS, FAST, V, PEER>;
-        if (MODE == 2) smem = scatter_smem_bytes<TILE_THREADS, ONEPASS_K>(sp.N, sp.stage_width, PEER, ALIGNED);
-        if (smem > 227 * 1024) return set_error(DFD_ERR_UNSUPPORTED, "k_scatter needs %zu B of shared memory per CTA", smem);
+        const size_t smem = scatter_smem_bytes<TILE_THREADS, K>(sp.N, sp.stage_width, PEER, ALIGNED);
+        if (smem > 227 * 1024)
+            return set_error(DFD_ERR_UNSUPPORTED, "num_partitions %u needs %zu B of shared memory per CTA (k_scatter)", sp.N, smem);
         if (smem > 48 * 1024) {
             if ((e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
                 return cuda_error(e, "cudaFuncSetAttribute(k_scatter)");
@@ -112,34 +115,33 @@ static int launch_scatter_kv(const ScatterParams& sp, int sm_count, size_t smem,
     return e == cudaSuccess ? DFD_OK : cuda_error(e, "k_scatter");
 }
 
-template <bool FAST, typename V, bool PEER, int MODE>
-static int launch_scatter_t(const ScatterParams& sp, int sm_count, size_t smem, cudaStream_t stream) {
-    if (use_aligned(sp.N, PEER)) return launch_scatter_kv<FAST, V, PEER, true, MODE>(sp, sm_count, smem, stream);
-    return launch_scatter_kv<FAST, V, PEER, false, MODE>(sp, sm_count, smem, stream);
+template <bool FAST, typename V, bool PEER, ScatterKind KIND>
+static int launch_scatter_t(const ScatterParams& sp, int sm_count, cudaStream_t stream) {
+    if (use_aligned(sp.N, PEER)) return launch_scatter_kv<FAST, V, PEER, true, KIND>(sp, sm_count, stream);
+    return launch_scatter_kv<FAST, V, PEER, false, KIND>(sp, sm_count, stream);
 }
 
-template <bool FAST, bool PEER, int MODE>
-static int launch_scatter_w(const ScatterParams& sp, int width, int sm_count, size_t smem, cudaStream_t stream) {
+template <bool FAST, bool PEER, ScatterKind KIND>
+static int launch_scatter_w(const ScatterParams& sp, int width, int sm_count, cudaStream_t stream) {
     switch (width) {
-        case 8: return launch_scatter_t<FAST, uint64_t, PEER, MODE>(sp, sm_count, smem, stream);
-        case 4: return launch_scatter_t<FAST, uint32_t, PEER, MODE>(sp, sm_count, smem, stream);
-        case 2: return launch_scatter_t<FAST, uint16_t, PEER, MODE>(sp, sm_count, smem, stream);
-        case 1: return launch_scatter_t<FAST, uint8_t, PEER, MODE>(sp, sm_count, smem, stream);
-        case 16: return launch_scatter_t<FAST, uint4, PEER, MODE>(sp, sm_count, smem, stream);
+        case 8: return launch_scatter_t<FAST, uint64_t, PEER, KIND>(sp, sm_count, stream);
+        case 4: return launch_scatter_t<FAST, uint32_t, PEER, KIND>(sp, sm_count, stream);
+        case 2: return launch_scatter_t<FAST, uint16_t, PEER, KIND>(sp, sm_count, stream);
+        case 1: return launch_scatter_t<FAST, uint8_t, PEER, KIND>(sp, sm_count, stream);
+        case 16: return launch_scatter_t<FAST, uint4, PEER, KIND>(sp, sm_count, stream);
         default:
-            if constexpr (PEER || MODE == 1) {
+            if constexpr (PEER || KIND == ScatterKind::OnePass) {
                 return set_error(DFD_ERR_INTERNAL, "bit-packed columns take the local k_scatter instantiation");
             } else {
-                return launch_scatter_t<FAST, BitColumn, false, MODE>(sp, sm_count, smem, stream);
+                return launch_scatter_t<FAST, BitColumn, false, KIND>(sp, sm_count, stream);
             }
     }
 }
 
-// one definition per translation unit (dfd_scatter_*.cu)
-template <bool PEER, int MODE>
-int launch_scatter_impl(const ScatterParams& sp, int width, bool fast, int sm_count, size_t smem, cudaStream_t stream) {
-    return fast ? launch_scatter_w<true, PEER, MODE>(sp, width, sm_count, smem, stream)
-                : launch_scatter_w<false, PEER, MODE>(sp, width, sm_count, smem, stream);
+template <bool PEER, ScatterKind KIND>
+int launch_scatter_impl(const ScatterParams& sp, int width, bool fast, int sm_count, cudaStream_t stream) {
+    return fast ? launch_scatter_w<true, PEER, KIND>(sp, width, sm_count, stream)
+                : launch_scatter_w<false, PEER, KIND>(sp, width, sm_count, stream);
 }
 
 }  // namespace dfd

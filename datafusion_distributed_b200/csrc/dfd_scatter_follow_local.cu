@@ -2,7 +2,5 @@
 #include "dfd_launch.cuh"
 
 namespace dfd {
-int launch_scatter_follow_local(const ScatterParams& sp, int width, bool fast, int sm_count, size_t smem, cudaStream_t stream) {
-    return launch_scatter_impl<false, 2>(sp, width, fast, sm_count, smem, stream);
-}
+template int launch_scatter_impl<false, ScatterKind::FollowUp>(const ScatterParams&, int, bool, int, cudaStream_t);
 }  // namespace dfd

@@ -2,7 +2,5 @@
 #include "dfd_launch.cuh"
 
 namespace dfd {
-int launch_scatter_twopass_peer(const ScatterParams& sp, int width, bool fast, int sm_count, size_t smem, cudaStream_t stream) {
-    return launch_scatter_impl<true, 0>(sp, width, fast, sm_count, smem, stream);
-}
+template int launch_scatter_impl<true, ScatterKind::TwoPass>(const ScatterParams&, int, bool, int, cudaStream_t);
 }  // namespace dfd
