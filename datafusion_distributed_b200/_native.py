@@ -68,7 +68,7 @@ class DfdMetrics(C.Structure):
 
 class DfdExecOptions(C.Structure):
     _fields_ = [("chunk_rows", C.c_int64), ("pipeline_depth", C.c_int32), ("pinned_pool_chunks", C.c_int32),
-                ("max_pinned_chunks", C.c_int32), ("reserved", C.c_int32)]
+                ("max_pinned_chunks", C.c_int32), ("device_output", C.c_int32)]
 
 
 class DfdExecStats(C.Structure):
@@ -97,6 +97,11 @@ class ArrowArrayStreamStruct(C.Structure):
 class ArrowDeviceArrayStruct(C.Structure):
     _fields_ = [("array", ArrowArrayStruct), ("device_id", C.c_int64), ("device_type", C.c_int32), ("sync_event", C.c_void_p),
                 ("reserved", C.c_int64 * 3)]
+
+
+class ArrowDeviceArrayStreamStruct(C.Structure):
+    _fields_ = [("device_type", C.c_int32), ("get_schema", C.c_void_p), ("get_next", C.c_void_p), ("get_last_error", C.c_void_p),
+                ("release", C.c_void_p), ("private_data", C.c_void_p)]
 
 
 # name -> (restype, argtypes).  Every symbol include/dfd_b200.h declares.
@@ -145,6 +150,8 @@ SIGNATURES = {
     "dfd_repartition_exec_abort": (C.c_int, [_VP, C.c_char_p]),
     "dfd_repartition_exec_run": (C.c_int, [_VP, C.POINTER(ArrowArrayStreamStruct)]),
     "dfd_repartition_exec_execute": (C.c_int, [_VP, C.c_uint32, C.POINTER(ArrowArrayStreamStruct)]),
+    "dfd_repartition_exec_execute_device": (C.c_int, [_VP, C.c_uint32, C.POINTER(ArrowDeviceArrayStreamStruct)]),
+    "dfd_repartition_exec_run_device": (C.c_int, [_VP, C.POINTER(ArrowDeviceArrayStreamStruct)]),
     "dfd_repartition_exec_stats": (C.c_int, [_VP, C.POINTER(DfdExecStats)]),
     "dfd_nccl_unique_id": (C.c_int, [_VP]),
     "dfd_exchange_create": (C.c_int, [_VP, C.c_int, C.c_int, _VP, C.POINTER(_VP)]),

@@ -9,7 +9,10 @@
 // GPU in chunks (H2D stream), partitioned by K1/K1b/K2 (compute stream), copied
 // back into pooled pinned memory (D2H stream) and handed out as zero-copy
 // per-destination slices — the three stages of consecutive chunks overlap, so
-// end-to-end time approaches max(H2D, D2H) over PCIe.
+// end-to-end time approaches max(H2D, D2H) over PCIe.  Input batches may also be
+// device-resident (push_device), and an operator created for device output keeps
+// its chunks on the GPU: the partition kernels write pooled DEVICE chunks in place
+// and the streams carry ArrowDeviceArray slices of them (execute_device).
 #include <cuda_runtime.h>
 
 #include <atomic>
@@ -133,10 +136,22 @@ struct SharedInput {
     }
 };
 
-// One D2H landing buffer (pinned): all columns of one chunk, destination-sorted.
+// All columns of one chunk, destination-sorted: the D2H landing buffer (pinned) of a host-output operator, or the buffers the
+// partition kernels write in place (device memory) of a device-output operator.
 struct OutChunk {
-    std::vector<void*> views;        // per column: 16-byte views of a Utf8View / BinaryView column (host, built at emission)
-    std::vector<int64_t> view_sizes; // per column: the "variadic buffer sizes" buffer of such an array (one data buffer)
+    bool device = false;             // device-output operator: every buffer below is device memory
+    cudaEvent_t event = nullptr;     // device chunks: recorded after the last kernel that writes the chunk (the batches' sync_event)
+    std::vector<void*> views;        // per column: 16-byte views of a Utf8View / BinaryView column (host chunks: built at emission)
+    std::vector<int64_t> view_sizes; // per column: the "variadic buffer sizes" buffer of such an array (one data buffer) ...
+    int64_t* d_view_sizes = nullptr; //   ... and where it lives for a device chunk (one int64 per column)
+    std::vector<const void*> child_off, child_valid;  // per list column: offsets / validity bitmap of its values array
+    std::vector<dfd::Scratch> list_tmp;  // device chunks, per list column: [child offsets | child validity bits | scan block sums]
+    struct Dict {                    // device chunks, host input: the chunk's dictionary of a column, uploaded once per chunk
+        dfd::Scratch mem;
+        ArrowArray array;            //   (shallow: length / offset / null_count of the input's; `buffers` point into mem)
+        std::vector<const void*> bufs;
+    };
+    std::vector<Dict> dicts;
     std::vector<std::shared_ptr<SharedInput>> inputs;  // input batches whose dictionaries this chunk's batches reference
     std::vector<void*> values;    // per column: values (fixed / bool) or string bytes (var-width, grown on demand)
     std::vector<void*> validity;  // per column (may be null)
@@ -146,14 +161,25 @@ struct OutChunk {
     std::shared_ptr<PinnedPool> pool;
 };
 
+// chunk memory of either kind
+cudaError_t chunk_alloc(bool device, void** p, size_t n) { return device ? cudaMalloc(p, n) : cudaHostAlloc(p, n, cudaHostAllocPortable); }
+void chunk_free(bool device, void* p) {
+    if (!p) return;
+    if (device) cudaFree(p);
+    else cudaFreeHost(p);
+}
+
 void destroy_out_chunk(OutChunk* c) {
-    for (void* p : c->values)
-        if (p) cudaFreeHost(p);
-    for (void* p : c->validity)
-        if (p) cudaFreeHost(p);
-    for (void* p : c->offsets)
-        if (p) cudaFreeHost(p);
-    for (void* p : c->views) free(p);
+    for (void* p : c->values) chunk_free(c->device, p);
+    for (void* p : c->validity) chunk_free(c->device, p);
+    for (void* p : c->offsets) chunk_free(c->device, p);
+    for (void* p : c->views)
+        if (c->device) cudaFree(p);
+        else free(p);
+    for (dfd::Scratch& t : c->list_tmp) cudaFree(t.ptr);
+    for (OutChunk::Dict& d : c->dicts) cudaFree(d.mem.ptr);
+    cudaFree(c->d_view_sizes);
+    if (c->event) cudaEventDestroy(c->event);
     delete c;
 }
 
@@ -210,6 +236,7 @@ std::shared_ptr<PinnedCache> pinned_cache_of(dfd_ctx* ctx) {  // caller holds no
     return std::static_pointer_cast<PinnedCache>(ctx->pinned_cache);
 }
 
+// The operator's pool of output chunks: pinned chunks, or device chunks for a device-output operator (same bound, same counters).
 struct PinnedPool : std::enable_shared_from_this<PinnedPool> {
     int device = 0;
     int64_t chunk_rows = 0;
@@ -219,6 +246,7 @@ struct PinnedPool : std::enable_shared_from_this<PinnedPool> {
     std::vector<OutChunk*> free_list;
     std::vector<OutChunk*> all;
     size_t max_chunks = 0;  // 0 = unbounded; otherwise acquire() blocks until a consumer returns a chunk (back-pressure)
+    bool device_out = false;  // the chunks are device memory, each with its event; they are not kept past the pool (no context cache)
     std::weak_ptr<PinnedCache> cache;  // the worker context's cache (gone once the context is destroyed)
     std::string layout;                // what makes two pools' chunks interchangeable: per field kind / width / nullable / view
     std::atomic<uint64_t> n_allocated{0}, n_reused{0};  // chunks pinned by this pool / taken over from the context's cache
@@ -274,6 +302,20 @@ struct PinnedPool : std::enable_shared_from_this<PinnedPool> {
         OutChunk* c = new (std::nothrow) OutChunk();
         if (!c) return nullptr;
         cudaSetDevice(device);
+        c->device = device_out;
+        c->child_off.assign(fields.size(), nullptr);
+        c->child_valid.assign(fields.size(), nullptr);
+        if (device_out) {
+            c->list_tmp.resize(fields.size());
+            c->dicts.resize(fields.size());
+            if (cudaEventCreateWithFlags(&c->event, cudaEventDisableTiming) != cudaSuccess ||
+                cudaMalloc((void**)&c->d_view_sizes, sizeof(int64_t) * fields.size()) != cudaSuccess) {
+                destroy_out_chunk(c);
+                return nullptr;
+            }
+        }
+        // (device chunks are what the scatter kernels write: sized like the slot's own output buffers of a host-output operator)
+        const size_t pad = device_out ? 8 : 0;
         for (const FieldInfo& f : fields) {
             void* v = nullptr;
             void* b = nullptr;
@@ -284,13 +326,19 @@ struct PinnedPool : std::enable_shared_from_this<PinnedPool> {
                 c->views.push_back(nullptr); c->view_sizes.push_back(0);
                 continue;
             }
-            if (!f.var() && cudaHostAlloc(&v, value_bytes(f, chunk_rows), cudaHostAllocPortable) != cudaSuccess) ok = false;
-            if (ok && (f.flags & ARROW_FLAG_NULLABLE) && cudaHostAlloc(&b, bitmap_bytes(chunk_rows), cudaHostAllocPortable) != cudaSuccess) ok = false;
-            if (ok && f.var() && cudaHostAlloc(&o, (size_t)(chunk_rows + 16) * f.ow(), cudaHostAllocPortable) != cudaSuccess) ok = false;
+            void* vw = nullptr;
+            const size_t vpad = device_out ? 16 * (size_t)(f.width ? f.width : 1) : 0;
+            if (!f.var() && chunk_alloc(device_out, &v, value_bytes(f, chunk_rows) + vpad) != cudaSuccess) ok = false;
+            if (ok && (f.flags & ARROW_FLAG_NULLABLE) && chunk_alloc(device_out, &b, bitmap_bytes(chunk_rows) + pad) != cudaSuccess) ok = false;
+            if (ok && f.var() && chunk_alloc(device_out, &o, (size_t)(chunk_rows + 16) * f.ow()) != cudaSuccess) ok = false;
+            if (ok && f.view) {
+                if (!device_out) vw = malloc((size_t)(chunk_rows + 16) * 16);
+                else if (cudaMalloc(&vw, (size_t)(chunk_rows + 16) * 16) != cudaSuccess) ok = false;
+            }
             if (!ok) {  // free what this chunk already holds: nothing leaks on a failed allocation
-                if (v) cudaFreeHost(v);
-                if (b) cudaFreeHost(b);
-                if (o) cudaFreeHost(o);
+                chunk_free(device_out, v);
+                chunk_free(device_out, b);
+                chunk_free(device_out, o);
                 destroy_out_chunk(c);
                 return nullptr;
             }
@@ -298,7 +346,7 @@ struct PinnedPool : std::enable_shared_from_this<PinnedPool> {
             c->validity.push_back(b);
             c->offsets.push_back(o);
             c->data_cap.push_back(0);
-            c->views.push_back(f.view ? malloc((size_t)(chunk_rows + 16) * 16) : nullptr);
+            c->views.push_back(vw);
             c->view_sizes.push_back(0);
         }
         n_allocated.fetch_add(1);
@@ -524,6 +572,7 @@ struct dfd_repartition_exec {
     std::vector<FieldTmp> tmp;
     // the first non-empty push decides whether the operator takes host (push) or device (push_device) batches
     int input_mode = INPUT_UNSET;
+    bool device_out = false;               // dfd_exec_options.device_output: chunks stay on the device, streams carry ArrowDeviceArray
     dfd::Scratch d_sizes;                  // device input: k_stage_sizes results, 4 x int64 per var-width column
     int64_t* h_sizes = nullptr;            // pinned: their read-back
     cudaEvent_t e_sizes = nullptr;
@@ -565,19 +614,26 @@ int emit_slot(dfd_repartition_exec* x, Slot& s) {
         XCUDA(x, cudaEventSynchronize(s.e_d2h), "D2H");
     }
     OutChunk* oc = s.out;
-    oc->inputs = std::move(s.dict_held);  // the output batches reference the inputs' dictionaries
+    if (!oc->device) {
+        oc->inputs = std::move(s.dict_held);  // the output batches reference the inputs' dictionaries
+    } else {
+        // a device batch cannot reference host memory: its dictionary is the device input batch's own (that batch lives until
+        // the chunk's last batch is released), or the copy flush_current uploaded into the chunk (host input)
+        oc->inputs.clear();
+        if (x->input_mode == INPUT_DEVICE && !s.dict_held.empty()) oc->inputs.push_back(s.held.back());
+    }
     s.held.clear();
     s.dict_held.clear();
     s.out = nullptr;
     s.in_flight = false;
     const size_t C = x->n_visible;  // the output batches carry the schema's columns; hidden list columns are folded into their list
-    for (size_t c = 0; c < C; ++c) {
-        if (!x->fields[c].list) continue;
+    for (size_t c = 0; c < C; ++c) {  // (a device chunk has had this loop and the next done by k_emit_chunk)
+        if (!x->fields[c].list || oc->device) continue;
         int32_t* lo32 = (int32_t*)oc->offsets[(size_t)x->fields[c].h_len];  // byte offsets into the 4-byte lengths -> element offsets
         for (int64_t r = 0; r <= s.rows; ++r) lo32[r] >>= 2;
     }
     for (size_t c = 0; c < C; ++c) {
-        if (!x->fields[c].view) continue;
+        if (!x->fields[c].view || oc->device) continue;
         // Utf8View output: 16-byte views over the chunk's single data buffer (inline when <= 12 bytes)
         const int32_t* off = (const int32_t*)oc->offsets[c];
         const int64_t rows = s.rows;
@@ -612,8 +668,8 @@ int emit_slot(dfd_repartition_exec* x, Slot& s) {
                 bp->child_bufs[4 * c + 1] = oc->offsets[hl];
                 ArrowArray& g = bp->grand[c];
                 memset(&g, 0, sizeof g);
-                bp->grand_bufs[3 * c] = f.h_valid >= 0 ? oc->values[(size_t)f.h_valid] : nullptr;
-                bp->grand_bufs[3 * c + 1] = f.child_width > 0 ? oc->values[hb] : oc->values[hl];  // primitive child: [validity, values]
+                bp->grand_bufs[3 * c] = f.h_valid >= 0 ? oc->child_valid[c] : nullptr;
+                bp->grand_bufs[3 * c + 1] = f.child_width > 0 ? oc->values[hb] : oc->child_off[c];  // primitive child: [validity, values]
                 bp->grand_bufs[3 * c + 2] = oc->values[hb];
                 g.length = s.col[hl].data_bytes / 4;
                 g.null_count = f.h_valid >= 0 ? -1 : 0;
@@ -636,20 +692,21 @@ int emit_slot(dfd_repartition_exec* x, Slot& s) {
             bp->child_bufs[4 * c] = hv ? oc->validity[c] : nullptr;
             bp->child_bufs[4 * c + 1] = f.view ? oc->views[c] : (var ? oc->offsets[c] : oc->values[c]);
             bp->child_bufs[4 * c + 2] = var ? oc->values[c] : nullptr;
-            bp->child_bufs[4 * c + 3] = f.view ? (const void*)&oc->view_sizes[c] : nullptr;
+            bp->child_bufs[4 * c + 3] = !f.view ? nullptr : oc->device ? (const void*)(oc->d_view_sizes + c) : (const void*)&oc->view_sizes[c];
             a.length = cnt;
             a.offset = start;  // zero-copy slice of the chunk-wide destination-sorted buffer
             a.null_count = hv ? -1 : 0;
             a.n_buffers = f.view ? 4 : (var ? 3 : 2);  // view arrays: validity, views, one data buffer, variadic buffer sizes
             a.buffers = &bp->child_bufs[4 * c];
             a.release = child_release;
-            if (f.dict && !oc->inputs.empty()) {
-                // the dictionary travels by reference: a shallow copy of the input batch's dictionary, kept alive by the shared input
-                const ArrowArray* src = oc->inputs.back()->array.children[c]->dictionary;
+            if (f.dict && (!oc->inputs.empty() || oc->device)) {
+                // the dictionary travels by reference: a shallow copy of the input batch's dictionary, kept alive by the shared
+                // input — or of the chunk's own uploaded copy, kept alive by the chunk
+                const ArrowArray* src = !oc->inputs.empty() ? oc->inputs.back()->array.children[c]->dictionary : &oc->dicts[c].array;
                 bp->dicts[c] = *src;
                 bp->dicts[c].release = dict_release;
                 bp->dicts[c].private_data = nullptr;
-                bp->dict_owner.push_back(oc->inputs.back());
+                if (!oc->inputs.empty()) bp->dict_owner.push_back(oc->inputs.back());
                 a.dictionary = &bp->dicts[c];
             }
             bp->child_ptrs[c] = &a;
@@ -676,7 +733,61 @@ int emit_slot(dfd_repartition_exec* x, Slot& s) {
     return DFD_OK;
 }
 
-// run the kernels + D2H for the chunk accumulated in the current slot
+// bytes of the values [0, offset + length) of dictionary `d`, which is in host memory
+size_t dict_value_bytes(const FieldInfo& f, const ArrowArray* d) {
+    const int64_t dn = d->offset + d->length;
+    if (f.dict_kind == DFD_COL_BOOL) return (size_t)((dn + 7) / 8);
+    if (!f.dict_var()) return (size_t)dn * f.dict_width;
+    return (size_t)(f.dict_ow() == 8 ? ((const int64_t*)d->buffers[1])[dn] : ((const int32_t*)d->buffers[1])[dn]);
+}
+
+// the string bytes of column i of a chunk need room for nb bytes (the buffer is never NULL, even for 0 bytes)
+int grow_chunk_bytes(dfd_repartition_exec* x, OutChunk* oc, size_t i, size_t nb) {
+    if (oc->data_cap[i] >= nb && oc->values[i]) return DFD_OK;
+    chunk_free(oc->device, oc->values[i]);
+    oc->values[i] = nullptr;
+    oc->data_cap[i] = 0;
+    const size_t want = (nb + nb / 4 + 64 + 15) & ~(size_t)15;
+    XCUDA(x, chunk_alloc(oc->device, &oc->values[i], want), "chunk allocation (string bytes)");
+    oc->data_cap[i] = want;
+    return DFD_OK;
+}
+
+// Device output, host input: every buffer of dictionary `d` (host memory) of column i goes to memory the chunk owns, once per
+// chunk, on the H2D stream.  Caller holds the context lock.
+int upload_dictionary(dfd_repartition_exec* x, OutChunk* oc, size_t i, const ArrowArray* d) {
+    const FieldInfo& f = x->fields[i];
+    const int64_t dn = d->offset + d->length, nbuf = d->n_buffers;
+    const bool view = f.dict_format[0] == 'v', dvar = !view && f.dict_var();
+    if (nbuf < (view || dvar ? 3 : 2) || !d->buffers || !d->buffers[1])
+        return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": malformed dictionary");
+    std::vector<size_t> nb((size_t)nbuf, 0);
+    if (d->null_count != 0 && d->buffers[0]) nb[0] = (size_t)((dn + 7) / 8);
+    nb[1] = f.dict_kind == DFD_COL_BOOL ? (size_t)((dn + 7) / 8) : view ? (size_t)dn * 16 : dvar ? (size_t)(dn + 1) * f.dict_ow() : (size_t)dn * f.dict_width;
+    if (dvar) nb[2] = dict_value_bytes(f, d);
+    if (view) {  // the variadic data buffers and, last, their sizes (on the device too)
+        for (int64_t k = 0; k + 3 < nbuf; ++k) nb[(size_t)k + 2] = (size_t)((const int64_t*)d->buffers[nbuf - 1])[k];
+        nb[(size_t)nbuf - 1] = (size_t)(nbuf - 3) * 8;
+    }
+    auto al = [](size_t v) { return (v + 16 + 255) & ~(size_t)255; };
+    size_t total = 0;
+    for (size_t n : nb) total += al(n);
+    OutChunk::Dict& od = oc->dicts[i];
+    if (int rc = od.mem.ensure(total, x->ctx->device)) return fail(x, rc, dfd_last_error());
+    od.bufs.assign((size_t)nbuf, nullptr);
+    char* at = (char*)od.mem.ptr;
+    for (size_t k = 0; k < (size_t)nbuf; at += al(nb[k]), ++k) {
+        if (!d->buffers[k] || (k == 0 && !nb[0])) continue;
+        if (nb[k]) XCUDA(x, cudaMemcpyAsync(at, d->buffers[k], nb[k], cudaMemcpyHostToDevice, x->s_h2d), "H2D dictionary");
+        x->bytes_h2d += nb[k];
+        od.bufs[k] = at;
+    }
+    od.array = *d;
+    od.array.buffers = od.bufs.data();
+    return DFD_OK;
+}
+
+// run the kernels + D2H for the chunk accumulated in the current slot (device output: the kernels write the chunk in place)
 int flush_current(dfd_repartition_exec* x) {
     if (!x->cur_open) return DFD_OK;
     Slot& s = x->slots[x->cur];
@@ -691,9 +802,19 @@ int flush_current(dfd_repartition_exec* x) {
         ScopedNs waited(x->ns_wait_pool);
         s.out = x->pool->acquire();
     }
-    if (!s.out) return fail(x, DFD_ERR_OOM, "pinned host allocation failed");
+    if (!s.out) return fail(x, DFD_ERR_OOM, x->device_out ? "device chunk allocation failed" : "pinned host allocation failed");
+    OutChunk* oc = s.out;
+    const bool dev = oc->device;
     std::lock_guard<std::mutex> lk(c->mu);
     XCUDA(x, cudaSetDevice(c->device), "cudaSetDevice");
+    if (dev) {
+        for (int fi : x->dev_fields)  // the scatter kernels write the chunk's own buffers: room for the string bytes first
+            if (x->fields[(size_t)fi].var())
+                if (int rc = grow_chunk_bytes(x, oc, (size_t)fi, (size_t)s.col[(size_t)fi].data_bytes)) return rc;
+        for (size_t i = 0; i < x->n_visible && x->input_mode == INPUT_HOST; ++i)
+            if (x->fields[i].dict && !s.dict_held.empty())
+                if (int rc = upload_dictionary(x, oc, i, s.dict_held.back()->array.children[i]->dictionary)) return rc;
+    }
     for (int fi : x->dev_fields) {  // the buffers concatenated on the host while staging: bitmaps and re-based offsets
         if (x->input_mode == INPUT_DEVICE) break;  // (device input: k_stage_batch built them in place)
         const FieldInfo& f = x->fields[(size_t)fi];
@@ -718,19 +839,23 @@ int flush_current(dfd_repartition_exec* x) {
     const size_t D = x->dev_fields.size();  // device columns: every field except the list placeholders (+ the hidden list columns)
     std::vector<dfd_column> in(D), out(D);
     for (size_t k = 0; k < D; ++k) {
-        const FieldInfo& f = x->fields[(size_t)x->dev_fields[k]];
-        const SlotCol& sc = s.col[(size_t)x->dev_fields[k]];
+        const size_t i = (size_t)x->dev_fields[k];
+        const FieldInfo& f = x->fields[i];
+        const SlotCol& sc = s.col[i];
+        // where the scatter kernels write: the slot's output buffers (copied to the pinned chunk below), or the device chunk itself
+        void* o_values = dev ? oc->values[i] : sc.d_out;
+        uint8_t* o_valid = !sc.has_valid ? nullptr : (uint8_t*)(dev ? oc->validity[i] : sc.d_out_valid);
         if (f.var()) {
             // (values_bytes = the bytes staged into this chunk: the offsets were built here, so the partitioner need not read them back)
             in[k] = dfd_column{f.kind, 0, sc.d_in, sc.d_in_off, sc.has_valid ? (uint8_t*)sc.d_in_valid : nullptr, 0, sc.data_bytes};
-            out[k] = dfd_column{f.kind, 0, sc.d_out, sc.d_out_off, sc.has_valid ? (uint8_t*)sc.d_out_valid : nullptr, 0, (int64_t)sc.out_cap};
+            out[k] = dfd_column{f.kind, 0, o_values, dev ? oc->offsets[i] : sc.d_out_off, o_valid, 0, (int64_t)(dev ? oc->data_cap[i] : sc.out_cap)};
         } else {
             in[k] = dfd_column{f.kind, f.width, sc.d_in, nullptr, sc.has_valid ? (uint8_t*)sc.d_in_valid : nullptr, 0, 0};
-            out[k] = dfd_column{f.kind, f.width, sc.d_out, nullptr, sc.has_valid ? (uint8_t*)sc.d_out_valid : nullptr, 0, 0};
+            out[k] = dfd_column{f.kind, f.width, o_values, nullptr, o_valid, 0, 0};
         }
         if (f.kind == DFD_COL_BOOL)
-            XCUDA(x, cudaMemsetAsync(sc.d_out, 0, PinnedPool::bitmap_bytes(s.rows), c->stream), "memset");
-        if (sc.has_valid) XCUDA(x, cudaMemsetAsync(sc.d_out_valid, 0, PinnedPool::bitmap_bytes(s.rows), c->stream), "memset");
+            XCUDA(x, cudaMemsetAsync(o_values, 0, PinnedPool::bitmap_bytes(s.rows), c->stream), "memset");
+        if (sc.has_valid) XCUDA(x, cudaMemsetAsync(o_valid, 0, PinnedPool::bitmap_bytes(s.rows), c->stream), "memset");
     }
     for (size_t i = 0; i < C; ++i)  // dictionary keys of this chunk (caller holds the context lock: set the fields directly)
         if (x->fields[i].dict && x->key_of_field[i] >= 0) {
@@ -742,6 +867,7 @@ int flush_current(dfd_repartition_exec* x) {
     // list fields: child offsets = exclusive scan of the gathered element lengths; child validity bytes -> bitmap
     std::vector<const void*> d2h_src(C, nullptr);
     std::vector<size_t> d2h_nb(C, 0);
+    auto scattered = [&](int field) -> void* { return dev ? oc->values[(size_t)field] : s.col[(size_t)field].d_out; };
     for (size_t i = 0; i < x->n_visible; ++i) {
         const FieldInfo& f = x->fields[i];
         if (!f.list) continue;
@@ -749,20 +875,25 @@ int flush_current(dfd_repartition_exec* x) {
         auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
         const size_t o_off = 0, o_bits = al((size_t)(ne + 1) * 4 + 16), o_sums = o_bits + al((size_t)(ne + 63) / 64 * 8 + 16);
         const size_t total = o_sums + al((size_t)(ne / 2048 + 4) * 8);
-        int rc2 = s.col[i].list_tmp.ensure(total, c->device);
+        dfd::Scratch& tmp = dev ? oc->list_tmp[i] : s.col[i].list_tmp;  // (a device chunk's batches point into it)
+        int rc2 = tmp.ensure(total, c->device);
         if (rc2) return fail(x, rc2, dfd_last_error());
-        char* lt = (char*)s.col[i].list_tmp.ptr;
+        char* lt = (char*)tmp.ptr;
+        if (dev) {
+            oc->child_off[i] = lt + o_off;
+            oc->child_valid[i] = lt + o_bits;
+        }
         if (f.child_width > 0) {  // primitive child: no child offsets; the gathered lengths themselves are not needed on the host
             d2h_src[(size_t)f.h_len] = lt + o_off;
             d2h_nb[(size_t)f.h_len] = 0;
         } else {
-            if ((rc2 = launch_lengths_to_offsets(s.col[(size_t)f.h_len].d_out, 4, ne, (unsigned long long*)(lt + o_sums), lt + o_off, c->stream)))
+            if ((rc2 = launch_lengths_to_offsets(scattered(f.h_len), 4, ne, (unsigned long long*)(lt + o_sums), lt + o_off, c->stream)))
                 return fail(x, rc2, dfd_last_error());
             d2h_src[(size_t)f.h_len] = lt + o_off;
             d2h_nb[(size_t)f.h_len] = (size_t)(ne + 1) * 4;
         }
         if (f.h_valid >= 0) {
-            if ((rc2 = launch_bytes_to_bits((const uint8_t*)s.col[(size_t)f.h_valid].d_out, ne, lt + o_bits, c->stream))) return fail(x, rc2, dfd_last_error());
+            if ((rc2 = launch_bytes_to_bits((const uint8_t*)scattered(f.h_valid), ne, lt + o_bits, c->stream))) return fail(x, rc2, dfd_last_error());
             d2h_src[(size_t)f.h_valid] = lt + o_bits;
             d2h_nb[(size_t)f.h_valid] = (size_t)((ne + 31) / 32 * 4);
         }
@@ -771,6 +902,35 @@ int flush_current(dfd_repartition_exec* x) {
           "D2H part_starts");
     XCUDA(x, cudaEventRecord(s.e_k, c->stream), "record k");
     s.k_recorded = true;
+    if (dev) {
+        // No D2H: what emission waits for is the copy of part_starts alone.  Views and list offsets are finished by one more
+        // kernel, and the chunk's own event, recorded behind it, is what the consumers of its batches wait on.
+        XCUDA(x, cudaEventRecord(s.e_d2h, c->stream), "record part_starts");
+        std::vector<EmitJob> jobs;
+        for (size_t i = 0; i < x->n_visible; ++i) {
+            const FieldInfo& f = x->fields[i];
+            EmitJob j;
+            j.n = s.rows;
+            if (f.view) {
+                j.off = oc->offsets[i];
+                j.bytes = oc->values[i];
+                j.dst = oc->views[i];
+                j.dst2 = oc->d_view_sizes + i;
+            } else if (f.list) {
+                j.op = EMIT_LIST_OFFSETS;
+                j.dst = oc->offsets[(size_t)f.h_len];
+            } else {
+                continue;
+            }
+            jobs.push_back(j);
+        }
+        if (!jobs.empty())
+            if (int rc2 = launch_emit_chunk(jobs.data(), (int)jobs.size(), c->stream)) return fail(x, rc2, dfd_last_error());
+        XCUDA(x, cudaEventRecord(oc->event, c->stream), "record chunk");
+        s.d2h_recorded = true;
+        s.in_flight = true;
+        return DFD_OK;
+    }
     // D2H of the destination-sorted chunk into the pooled pinned buffer taken above
     XCUDA(x, cudaStreamWaitEvent(x->s_d2h, s.e_k, 0), "wait k");
     for (size_t k = 0; k < D; ++k) {
@@ -782,14 +942,7 @@ int flush_current(dfd_repartition_exec* x) {
         if (f.var()) {
             nb = (size_t)sc.data_bytes;
             if (d2h_src[i]) { src = d2h_src[i]; nb = d2h_nb[i]; }  // list columns: scanned child offsets / re-packed child validity
-            if (s.out->data_cap[i] < nb || !s.out->values[i]) {  // grow this pinned chunk's string buffer (never NULL, even for 0 bytes)
-                if (s.out->values[i]) cudaFreeHost(s.out->values[i]);
-                s.out->values[i] = nullptr;
-                s.out->data_cap[i] = 0;
-                size_t want = nb + nb / 4 + 64;
-                XCUDA(x, cudaHostAlloc(&s.out->values[i], want, cudaHostAllocPortable), "cudaHostAlloc(string bytes)");
-                s.out->data_cap[i] = want;
-            }
+            if (int rc2 = grow_chunk_bytes(x, oc, i, nb)) return rc2;
             if (!f.hidden || f.role == 1) {  // (the per-row offsets of the hidden bytes / validity columns are not needed on the host)
                 XCUDA(x, cudaMemcpyAsync(s.out->offsets[i], sc.d_out_off, (size_t)(s.rows + 1) * f.ow(), cudaMemcpyDeviceToHost, x->s_d2h), "D2H offsets");
                 x->bytes_d2h += (size_t)(s.rows + 1) * f.ow();
@@ -802,6 +955,11 @@ int flush_current(dfd_repartition_exec* x) {
             x->bytes_d2h += (size_t)((s.rows + 7) / 8);
         }
     }
+    for (size_t i = 0; i < x->n_visible; ++i)  // the values arrays of list columns: scanned offsets / re-packed validity, as copied above
+        if (x->fields[i].list) {
+            oc->child_off[i] = oc->values[(size_t)x->fields[i].h_len];
+            oc->child_valid[i] = x->fields[i].h_valid >= 0 ? oc->values[(size_t)x->fields[i].h_valid] : nullptr;
+        }
     XCUDA(x, cudaEventRecord(s.e_d2h, x->s_d2h), "record d2h");
     s.d2h_recorded = true;
     s.in_flight = true;
@@ -902,6 +1060,7 @@ int grow_var_bytes(dfd_repartition_exec* x, int64_t n, bool* fits) {
         sc.d_out = nullptr;
         sc.in_cap = want;
         sc.out_cap = 0;
+        if (x->device_out) continue;  // (the scatter writes the chunk's own buffer, grown when the chunk is flushed)
         XCUDA(x, cudaMalloc(&sc.d_out, want), "cudaMalloc(string bytes)");
         sc.out_cap = want;
     }
@@ -1074,14 +1233,6 @@ int prepare_rows(dfd_repartition_exec* x, const ArrowArray* b, const HeldInput& 
 }
 
 size_t dict_hash_bytes(int64_t length) { return (size_t)(length + 1) * 8; }
-
-// bytes of the values [0, offset + length) of dictionary `d`, which is in host memory
-size_t dict_value_bytes(const FieldInfo& f, const ArrowArray* d) {
-    const int64_t dn = d->offset + d->length;
-    if (f.dict_kind == DFD_COL_BOOL) return (size_t)((dn + 7) / 8);
-    if (!f.dict_var()) return (size_t)dn * f.dict_width;
-    return (size_t)(f.dict_ow() == 8 ? ((const int64_t*)d->buffers[1])[dn] : ((const int32_t*)d->buffers[1])[dn]);
-}
 
 // Dictionary KEY field i: hash its values once per chunk on the device (DataFusion hash_dictionary); the chunk's rows pick
 // dict_hashes[index].  `values` are in device memory; the hashes go to the front of the slot's dict_buf (host input copies
@@ -1478,7 +1629,7 @@ void release_device_inputs(dfd_repartition_exec* x) {
 }
 
 // The device and pinned buffers of one pipeline slot: offsets and bitmaps for a full chunk now, string bytes on demand
-// (caller holds the context lock).  free_slot frees whatever it holds.
+// (caller holds the context lock).  A device-output operator has no d_out* buffers: its scatter writes the chunk.  free_slot frees whatever it holds.
 cudaError_t alloc_slot(const dfd_repartition_exec* x, Slot& s) {
     s.col.resize(x->fields.size());
     const size_t bitmap = PinnedPool::bitmap_bytes(x->chunk_rows) + 8;
@@ -1491,15 +1642,15 @@ cudaError_t alloc_slot(const dfd_repartition_exec* x, Slot& s) {
             const size_t ob = (size_t)(x->chunk_rows + 16) * f.ow();
             e = cudaMalloc(&sc.d_in_off, ob);
             if (e == cudaSuccess) e = cudaHostAlloc((void**)&sc.h_off, ob, cudaHostAllocPortable);
-            if (e == cudaSuccess) e = cudaMalloc(&sc.d_out_off, ob);
+            if (e == cudaSuccess && !x->device_out) e = cudaMalloc(&sc.d_out_off, ob);
         } else {
             const size_t vb = PinnedPool::value_bytes(f, x->chunk_rows) + 16 * (size_t)(f.width ? f.width : 1);
             e = cudaMalloc(&sc.d_in, vb);
-            if (e == cudaSuccess) e = cudaMalloc(&sc.d_out, vb);
+            if (e == cudaSuccess && !x->device_out) e = cudaMalloc(&sc.d_out, vb);
         }
         if (e == cudaSuccess && (f.flags & ARROW_FLAG_NULLABLE)) {
             e = cudaMalloc(&sc.d_in_valid, bitmap);
-            if (e == cudaSuccess) e = cudaMalloc(&sc.d_out_valid, bitmap);
+            if (e == cudaSuccess && !x->device_out) e = cudaMalloc(&sc.d_out_valid, bitmap);
         }
         if (e != cudaSuccess) return e;
     }
@@ -1611,6 +1762,30 @@ int push_rows(dfd_repartition_exec* x, ArrowArray* a, int mode, void* sync_event
     return DFD_OK;
 }
 
+ArrowArray& array_of(ArrowArray& a) { return a; }
+ArrowArray& array_of(ArrowDeviceArray& a) { return a.array; }
+
+// run and run_device: pull `input` to exhaustion through `push`, release it, finish
+template <typename Stream, typename Batch>
+int pull_stream(dfd_repartition_exec* x, Stream* input, int (*push)(dfd_repartition_exec*, Batch*)) {
+    int rc = DFD_OK;
+    for (;;) {
+        Batch a;
+        memset(&a, 0, sizeof a);
+        int e = input->get_next(input, &a);
+        if (e != 0) {
+            const char* m = input->get_last_error ? input->get_last_error(input) : nullptr;
+            rc = fail(x, DFD_ERR_INTERNAL, std::string("input stream error: ") + (m ? m : "unknown"));
+            if (x->input_mode == INPUT_DEVICE) release_device_inputs(x);
+            break;
+        }
+        if (!array_of(a).release) break;  // end of stream
+        if ((rc = push(x, &a))) break;
+    }
+    if (input->release) input->release(input);
+    if (rc) return rc;
+    return dfd_repartition_exec_finish(x);
+}
 }  // namespace
 
 extern "C" {
@@ -1715,6 +1890,11 @@ int dfd_repartition_exec_create(dfd_ctx* ctx, const struct ArrowSchema* schema, 
     if (!x) return set_error(DFD_ERR_OOM, "out of host memory");
     x->ctx = ctx;
     x->N = num_partitions;
+    if (opts && opts->device_output != 0 && opts->device_output != 1)
+        return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_exec_options.device_output is %d: 0 (host output) or 1 (device output)", (int)opts->device_output);
+    x->device_out = opts && opts->device_output == 1;
+    if (x->device_out && !launch_emit_chunk)  // (weak: see dfd_internal.h)
+        return set_error(DFD_ERR_UNSUPPORTED, "device output: this build of the operator has no emit kernel (dfd_emit.cu)");
     for (int64_t i = 0; i < schema->n_children; ++i) {  // (the same rules the plan hook checks through dfd_repartition_supported)
         int key_index = -1;
         for (int k = 0; k < n_keys; ++k)
@@ -1792,15 +1972,17 @@ int dfd_repartition_exec_create(dfd_ctx* ctx, const struct ArrowSchema* schema, 
     x->pool->device = ctx->device;
     x->pool->chunk_rows = x->chunk_rows;
     x->pool->set_fields(x->fields);
-    x->pool->cache = pinned_cache_of(ctx);
+    x->pool->device_out = x->device_out;
+    if (!x->device_out) x->pool->cache = pinned_cache_of(ctx);
     x->pool->max_chunks = (opts && opts->max_pinned_chunks > 0) ? (size_t)opts->max_pinned_chunks : 0;
     if (x->pool->max_chunks && x->pool->max_chunks < (size_t)pool_chunks) x->pool->max_chunks = (size_t)pool_chunks;
     std::vector<OutChunk*> pre;
     for (int i = 0; i < pool_chunks; ++i) {
         OutChunk* c = x->pool->acquire();
         if (!c) {
+            const bool device_out = x->device_out;
             dfd_repartition_exec_destroy(x.release());
-            return set_error(DFD_ERR_OOM, "pinned pool allocation failed");
+            return set_error(DFD_ERR_OOM, device_out ? "device chunk pool allocation failed" : "pinned pool allocation failed");
         }
         pre.push_back(c);
     }
@@ -1883,22 +2065,17 @@ int dfd_repartition_exec_abort(dfd_repartition_exec* x, const char* message) {
 
 int dfd_repartition_exec_run(dfd_repartition_exec* x, struct ArrowArrayStream* input) {
     if (!x || !input || !input->get_next) return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_repartition_exec_run: NULL argument");
-    int rc = DFD_OK;
-    for (;;) {
-        ArrowArray a;
-        memset(&a, 0, sizeof a);
-        int e = input->get_next(input, &a);
-        if (e != 0) {
-            const char* m = input->get_last_error ? input->get_last_error(input) : nullptr;
-            rc = fail(x, DFD_ERR_INTERNAL, std::string("input stream error: ") + (m ? m : "unknown"));
-            break;
-        }
-        if (!a.release) break;  // end of stream
-        if ((rc = dfd_repartition_exec_push(x, &a))) break;
+    return pull_stream(x, input, dfd_repartition_exec_push);
+}
+
+int dfd_repartition_exec_run_device(dfd_repartition_exec* x, struct ArrowDeviceArrayStream* input) {
+    if (!x || !input || !input->get_next) return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_repartition_exec_run_device: NULL argument");
+    if (input->device_type != ARROW_DEVICE_CUDA) {
+        const int type = (int)input->device_type;
+        if (input->release) input->release(input);
+        return set_error(DFD_ERR_INVALID_ARGUMENT, "device stream of device type %d: the operator takes CUDA streams", type);
     }
-    if (input->release) input->release(input);
-    if (rc) return rc;
-    return dfd_repartition_exec_finish(x);
+    return pull_stream(x, input, dfd_repartition_exec_push_device);
 }
 
 /* ---- output streams (ArrowArrayStream per destination) ------------------- */
@@ -1915,8 +2092,8 @@ int os_get_schema(ArrowArrayStream* s, ArrowSchema* out) {
     return export_schema(p->x->fields, out);
 }
 
-int os_get_next(ArrowArrayStream* s, ArrowArray* out) {
-    OutStreamPriv* p = (OutStreamPriv*)s->private_data;
+// the next batch of the stream's destination (blocking); *out is released (release == NULL) at the end of the stream
+int next_batch(OutStreamPriv* p, ArrowArray* out) {
     dfd_repartition_exec* x = p->x;
     std::unique_lock<std::mutex> lk(x->mu);
     PartQueue& q = x->queues[p->partition];
@@ -1934,6 +2111,30 @@ int os_get_next(ArrowArrayStream* s, ArrowArray* out) {
     return 0;
 }
 
+int os_get_next(ArrowArrayStream* s, ArrowArray* out) { return next_batch((OutStreamPriv*)s->private_data, out); }
+
+// The device streams hand out the same queued batches, wrapped: the buffers of a device-output operator's chunks are device
+// memory, and the chunk's event says when they are written.
+int ds_get_schema(ArrowDeviceArrayStream* s, ArrowSchema* out) { return export_schema(((OutStreamPriv*)s->private_data)->x->fields, out); }
+int ds_get_next(ArrowDeviceArrayStream* s, ArrowDeviceArray* out) {
+    OutStreamPriv* p = (OutStreamPriv*)s->private_data;
+    memset(out, 0, sizeof *out);
+    if (int e = next_batch(p, &out->array)) return e;
+    if (!out->array.release) return 0;
+    out->device_id = p->x->ctx->device;
+    out->device_type = ARROW_DEVICE_CUDA;
+    out->sync_event = &((BatchPriv*)out->array.private_data)->chunk->event;
+    return 0;
+}
+const char* ds_last_error(ArrowDeviceArrayStream* s) {
+    OutStreamPriv* p = (OutStreamPriv*)s->private_data;
+    return p->last_error.empty() ? nullptr : p->last_error.c_str();
+}
+void ds_release(ArrowDeviceArrayStream* s) {
+    delete (OutStreamPriv*)s->private_data;
+    s->release = nullptr;
+}
+
 const char* os_last_error(ArrowArrayStream* s) {
     OutStreamPriv* p = (OutStreamPriv*)s->private_data;
     return p->last_error.empty() ? nullptr : p->last_error.c_str();
@@ -1948,12 +2149,29 @@ void os_release(ArrowArrayStream* s) {
 int dfd_repartition_exec_execute(dfd_repartition_exec* x, uint32_t partition, struct ArrowArrayStream* out) {
     if (!x || !out) return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_repartition_exec_execute: NULL argument");
     if (partition >= x->N) return set_error(DFD_ERR_INVALID_ARGUMENT, "partition %u out of range [0,%u)", partition, x->N);
+    if (x->device_out) return set_error(DFD_ERR_INVALID_ARGUMENT, "execute on a device-output operator: its streams are taken with execute_device");
     OutStreamPriv* p = new (std::nothrow) OutStreamPriv{x, partition, {}};
     if (!p) return set_error(DFD_ERR_OOM, "out of host memory");
     out->get_schema = os_get_schema;
     out->get_next = os_get_next;
     out->get_last_error = os_last_error;
     out->release = os_release;
+    out->private_data = p;
+    return DFD_OK;
+}
+
+int dfd_repartition_exec_execute_device(dfd_repartition_exec* x, uint32_t partition, struct ArrowDeviceArrayStream* out) {
+    if (!x || !out) return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_repartition_exec_execute_device: NULL argument");
+    if (partition >= x->N) return set_error(DFD_ERR_INVALID_ARGUMENT, "partition %u out of range [0,%u)", partition, x->N);
+    if (!x->device_out)
+        return set_error(DFD_ERR_INVALID_ARGUMENT, "execute_device on a host-output operator: create it with dfd_exec_options.device_output = 1");
+    OutStreamPriv* p = new (std::nothrow) OutStreamPriv{x, partition, {}};
+    if (!p) return set_error(DFD_ERR_OOM, "out of host memory");
+    out->device_type = ARROW_DEVICE_CUDA;
+    out->get_schema = ds_get_schema;
+    out->get_next = ds_get_next;
+    out->get_last_error = ds_last_error;
+    out->release = ds_release;
     out->private_data = p;
     return DFD_OK;
 }

@@ -231,6 +231,25 @@ struct StageSize {
 };
 __attribute__((weak)) int launch_stage_sizes(const StageSize* jobs, int n_jobs, cudaStream_t s);
 
+// Device-resident OUTPUT (dfd_repartition_exec_execute_device; kernel in dfd_emit.cu): what the host does per row when it
+// finishes a host chunk, done on the device for a device chunk — all view and list columns of a chunk in one launch.
+enum EmitOp : int32_t {
+    EMIT_VIEWS = 0,        // int32 off[0, n] + bytes -> n 16-byte views at dst (bit-identical to host::build_views) and the
+                           //   int64 variadic buffer size off[n] at dst2
+    EMIT_LIST_OFFSETS = 1, // dst[r] >>= 2, r in [0, n]: byte offsets into the 4-byte lengths -> element offsets (int32, in place)
+};
+struct EmitJob {
+    int32_t op = EMIT_VIEWS, pad = 0;
+    const void* off = nullptr;    // views: int32 offsets
+    const void* bytes = nullptr;  // views: the string bytes, a 4-byte aligned buffer of off[n] bytes
+    void* dst = nullptr;
+    void* dst2 = nullptr;
+    int64_t n = 0;
+};
+// Weak like the staging launches: without dfd_emit.cu the operator object still links, and creating a device-output operator
+// fails with DFD_ERR_UNSUPPORTED.  libdfd_b200.so always links it.
+__attribute__((weak)) int launch_emit_chunk(const EmitJob* jobs, int n_jobs, cudaStream_t s);
+
 // Aligned write-out (k_scatter KV > K) is used for the peer-store exchange at small N (full-size NVLink write packets).
 bool use_aligned(uint32_t N, bool peer);
 // One scatter launch of a width group (template in dfd_launch.cuh).  Each (PEER, KIND) is instantiated in a translation unit

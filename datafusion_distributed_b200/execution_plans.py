@@ -4,7 +4,8 @@
 reference builds it (src/execution_plans/network_shuffle.rs:126-134) and runs
 it on every producer task (src/worker/impl_execute_task.rs:77-86):
 `execute(partition)` returns the stream of that destination's record batches.
-Host Arrow batches in, host Arrow batches out; the work happens on the GPU.
+Host Arrow batches in, host Arrow batches out; the work happens on the GPU.  Batches may also be device-resident on
+either side (`push_device_batch` / `run_device`, `device_output=True` + `execute_device`).
 """
 from __future__ import annotations
 
@@ -65,18 +66,78 @@ class PinnedTable:
             pass
 
 
+class DeviceBatchStream:
+    """Iterator over an Arrow C Device stream (`struct ArrowDeviceArrayStream`) of one destination's batches.  Each item is an
+    owned `ArrowDeviceArrayStruct`; it is released when the next one is asked for (or on `close`), so a consumer finishes
+    its device reads of a batch (after waiting on its `sync_event`) before it moves on."""
+
+    def __init__(self, stream: "nv.ArrowDeviceArrayStreamStruct"):
+        self._cs = stream
+        self._last = None
+
+    @property
+    def device_type(self) -> int:
+        return self._cs.device_type
+
+    @property
+    def schema(self):
+        import pyarrow as pa
+
+        out = nv.ArrowSchemaStruct()
+        rc = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p)(self._cs.get_schema)(C.addressof(self._cs), C.addressof(out))
+        if rc:
+            raise OSError(rc, "get_schema failed")
+        return pa.Schema._import_from_c(C.addressof(out))
+
+    def __iter__(self):
+        return self
+
+    def _release_last(self):
+        if self._last is not None and self._last.array.release:
+            C.CFUNCTYPE(None, C.c_void_p)(self._last.array.release)(C.addressof(self._last.array))
+        self._last = None
+
+    def __next__(self):
+        self._release_last()
+        if not self._cs.release:
+            raise StopIteration
+        out = nv.ArrowDeviceArrayStruct()
+        rc = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p)(self._cs.get_next)(C.addressof(self._cs), C.addressof(out))
+        if rc:
+            msg = C.CFUNCTYPE(C.c_char_p, C.c_void_p)(self._cs.get_last_error)(C.addressof(self._cs))
+            text = msg.decode("utf-8", "replace") if msg else "unknown"
+            self.close()
+            raise OSError(rc, text)
+        if not out.array.release:
+            self.close()
+            raise StopIteration
+        self._last = out
+        return out
+
+    def close(self):
+        self._release_last()
+        if self._cs.release:
+            C.CFUNCTYPE(None, C.c_void_p)(self._cs.release)(C.addressof(self._cs))
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class RepartitionExec:
     """`RepartitionExec::try_new(input, Partitioning::Hash(exprs, n))` on one GPU worker."""
 
     def __init__(self, ctx: WorkerContext, schema, partitioning: Partitioning, chunk_rows: int = 0,
-                 pipeline_depth: int = 0, pinned_pool_chunks: int = 0, max_pinned_chunks: int = 0):
+                 pipeline_depth: int = 0, pinned_pool_chunks: int = 0, max_pinned_chunks: int = 0, device_output: bool = False):
         self.ctx = ctx
         self.schema = schema
         self.partitioning = partitioning
         cs = nv.ArrowSchemaStruct()
         schema._export_to_c(C.addressof(cs))
         keys = (C.c_int32 * len(partitioning.key_cols))(*partitioning.key_cols)
-        opts = nv.DfdExecOptions(chunk_rows, pipeline_depth, pinned_pool_chunks, max_pinned_chunks, 0)
+        opts = nv.DfdExecOptions(chunk_rows, pipeline_depth, pinned_pool_chunks, max_pinned_chunks, 1 if device_output else 0)
         self._h = C.c_void_p()
         try:
             nv.check(nv.lib().dfd_repartition_exec_create(ctx.handle, C.byref(cs), keys, len(partitioning.key_cols),
@@ -126,6 +187,19 @@ class RepartitionExec:
         cs = nv.ArrowArrayStreamStruct()
         nv.check(nv.lib().dfd_repartition_exec_execute(self._h, partition, C.byref(cs)))
         return pa.RecordBatchReader._import_from_c(C.addressof(cs))
+
+    def run_device(self, device_stream):
+        """Pull an Arrow C Device stream (a pointer, int or ctypes, to a `struct ArrowDeviceArrayStream` of CUDA batches on this
+        worker's GPU) to exhaustion, then finish.  The stream is released, whatever the outcome."""
+        addr = device_stream if isinstance(device_stream, int) else C.addressof(device_stream)
+        nv.check(nv.lib().dfd_repartition_exec_run_device(self._h, C.cast(C.c_void_p(addr), C.POINTER(nv.ArrowDeviceArrayStreamStruct))))
+
+    def execute_device(self, partition: int) -> DeviceBatchStream:
+        """`execute(partition)` of an operator created with `device_output=True`: that destination's batches as
+        `ArrowDeviceArrayStruct`s whose buffers are in this worker's GPU memory."""
+        cs = nv.ArrowDeviceArrayStreamStruct()
+        nv.check(nv.lib().dfd_repartition_exec_execute_device(self._h, partition, C.byref(cs)))
+        return DeviceBatchStream(cs)
 
     def stats(self) -> dict:
         st = nv.DfdExecStats()

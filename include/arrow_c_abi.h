@@ -1,8 +1,9 @@
 /*
- * Arrow C Data / C Stream / C Device Data Interface structure definitions.
- * These are the published, frozen ABI structs of the Apache Arrow format
- * specification (docs: "The Arrow C data interface", "C stream interface",
- * "C device data interface"); every Arrow implementation (arrow-rs `ffi`,
+ * Arrow C Data / C Stream / C Device Data / C Device Stream Interface structure
+ * definitions.  These are the published, frozen ABI structs of the Apache Arrow
+ * format specification (docs: "The Arrow C data interface", "C stream interface",
+ * "C device data interface" and its "device stream interface"); every Arrow
+ * implementation (arrow-rs `ffi`,
  * pyarrow `_import_from_c/_export_to_c`) binds to exactly this layout.
  * The guards are the ones the specification mandates so this header can be
  * included next to any other copy.
@@ -80,6 +81,20 @@ struct ArrowDeviceArray {
 };
 
 #endif /* ARROW_C_DEVICE_DATA_INTERFACE */
+
+#ifndef ARROW_C_DEVICE_STREAM_INTERFACE
+#define ARROW_C_DEVICE_STREAM_INTERFACE
+
+struct ArrowDeviceArrayStream {
+    ArrowDeviceType device_type;
+    int (*get_schema)(struct ArrowDeviceArrayStream*, struct ArrowSchema* out);
+    int (*get_next)(struct ArrowDeviceArrayStream*, struct ArrowDeviceArray* out);
+    const char* (*get_last_error)(struct ArrowDeviceArrayStream*);
+    void (*release)(struct ArrowDeviceArrayStream*);
+    void* private_data;
+};
+
+#endif /* ARROW_C_DEVICE_STREAM_INTERFACE */
 
 #ifdef __cplusplus
 }

@@ -296,7 +296,10 @@ typedef struct {
                                    > 0 = hard bound: push()/finish() BLOCK until a consumer releases a chunk — the
                                    operator's back-pressure (needs concurrent consumers, like the reference's bounded
                                    hand-off, src/worker/worker_connection_pool.rs:151-153) */
-    int32_t reserved;
+    int32_t device_output;      /* 0 = the partition streams carry HOST batches (execute); 1 = they carry DEVICE batches
+                                   (execute_device): the kind of output is fixed when the operator is created, because the
+                                   first chunk is flushed before any stream is opened.  For a device-output operator
+                                   pinned_pool_chunks / max_pinned_chunks count device chunks */
 } dfd_exec_options;
 
 typedef struct {
@@ -331,7 +334,8 @@ int dfd_repartition_exec_push(dfd_repartition_exec* x, struct ArrowArray* batch)
  *     push of the other kind releases its batch and fails the operator with DFD_ERR_INVALID_ARGUMENT.
  *   - The partition streams are identical to those push() gives for the same batch contents (batches and their
  *     boundaries, row order, values incl. the bytes under null slots, validity, offsets, views, dictionaries, lists).
- *     Output batches are host arrays; a dictionary column references a HOST copy of the dictionary values.
+ *     Output batches of a host-output operator are host arrays; a dictionary column references a HOST copy of the
+ *     dictionary values.  (A device-output operator references the batch's own device dictionary: execute_device.)
  *   - dfd_exec_stats: rows_in counts the rows, bytes_h2d stays 0, dictionaries copied to the host count in bytes_d2h.
  *     Schemas with variable-width, view or list columns read each batch's byte counts back (one small D2H and one
  *     wait per batch); fixed-width / boolean / dictionary-index-only schemas never wait for the device while pushing,
@@ -345,6 +349,37 @@ int dfd_repartition_exec_finish(dfd_repartition_exec* x);
 int dfd_repartition_exec_abort(dfd_repartition_exec* x, const char* message);
 int dfd_repartition_exec_run(dfd_repartition_exec* x, struct ArrowArrayStream* input);
 int dfd_repartition_exec_execute(dfd_repartition_exec* x, uint32_t partition, struct ArrowArrayStream* out);
+/* DEVICE-resident output (Arrow C Device stream interface), for consumers that are on the GPU too: an operator created
+ * with dfd_exec_options.device_output = 1 hands out, per destination, a stream of ArrowDeviceArray record batches whose
+ * every buffer is in the context's GPU memory.  No payload byte crosses PCIe and the host builds no per-row structure.
+ * Replaces the same `ExecutionPlan::execute(partition, ctx) -> SendableRecordBatchStream` (src/worker/impl_execute_task.rs:77-86)
+ * as execute, for a consumer that reads GPU memory.
+ *   - out->device_type == ARROW_DEVICE_CUDA; get_schema gives what execute's stream gives; get_next blocks like the host
+ *     stream's and ends with a released array (array.release == NULL); an operator error or abort arrives as EIO +
+ *     get_last_error on every partition stream, after the batches already queued.
+ *   - execute on a device-output operator and execute_device on a host-output one fail with DFD_ERR_INVALID_ARGUMENT.
+ *   - Every batch: device_type == ARROW_DEVICE_CUDA, device_id == the context's device, and sync_event points to a
+ *     cudaEvent_t recorded on the compute stream after the last kernel that writes the batch's chunk.  The consumer makes
+ *     its stream wait on it (cudaStreamWaitEvent) before reading; the library never makes the host wait for it.  The
+ *     event belongs to the chunk and stays valid until the batch is released.
+ *   - Batches are zero-copy slices (offset, length) of chunk-wide destination-sorted DEVICE buffers, with the batch
+ *     boundaries, offsets, lengths, null counts and buffer contents (the bytes under null slots, all 16 bytes of every
+ *     view, list offsets and children) of the host stream for the same input.  View arrays carry their variadic-sizes
+ *     buffer in device memory.  Dictionaries are device-resident: with device input they are the input batch's own
+ *     (a device input batch that carries dictionaries is therefore released when the last output batch referencing it is
+ *     released, not at finish()); with host input the chunk's dictionary is uploaded once per chunk (counted in bytes_h2d).
+ *   - Ownership: the consumer owns each batch and releases it AFTER its device reads of the batch have completed; the
+ *     release of a chunk's last batch returns the chunk to the operator's pool.  With max_pinned_chunks, push / finish
+ *     block until a consumer releases a chunk, as for pinned chunks.
+ *   - dfd_exec_stats: device input + device output of a fixed-width / Boolean schema moves nothing over PCIe
+ *     (bytes_h2d == 0 and bytes_d2h == 0); dictionary copies made to compare dictionaries at chunk cuts and the size
+ *     read-backs of device input still count in bytes_d2h. */
+int dfd_repartition_exec_execute_device(dfd_repartition_exec* x, uint32_t partition, struct ArrowDeviceArrayStream* out);
+/* The device twin of run: pulls `input` (an Arrow C Device stream of ARROW_DEVICE_CUDA batches on the context's device) to
+ * exhaustion through push_device, then finishes.  A stream of another device type is refused with
+ * DFD_ERR_INVALID_ARGUMENT; a get_next error aborts the operator with the stream's message.  The stream is released
+ * exactly once, whatever the outcome. */
+int dfd_repartition_exec_run_device(dfd_repartition_exec* x, struct ArrowDeviceArrayStream* input);
 int dfd_repartition_exec_stats(dfd_repartition_exec* x, dfd_exec_stats* out);
 
 /* ---- inter-worker exchange (one worker per GPU, single NVSwitch box) -------

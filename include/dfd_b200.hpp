@@ -131,6 +131,10 @@ public:
     void run(ArrowArrayStream* input) { check(dfd_repartition_exec_run(h_, input)); }
     // ≙ ExecutionPlan::execute(partition, ctx) -> SendableRecordBatchStream
     void execute(uint32_t partition, ArrowArrayStream* out) { check(dfd_repartition_exec_execute(h_, partition, out)); }
+    // device-resident batches in / out (an operator created with dfd_exec_options.device_output = 1 for the output side)
+    void push_device_batch(ArrowDeviceArray* batch) { check(dfd_repartition_exec_push_device(h_, batch)); }  // ownership moves
+    void run_device(ArrowDeviceArrayStream* input) { check(dfd_repartition_exec_run_device(h_, input)); }
+    void execute_device(uint32_t partition, ArrowDeviceArrayStream* out) { check(dfd_repartition_exec_execute_device(h_, partition, out)); }
 
 private:
     Partitioning partitioning_;

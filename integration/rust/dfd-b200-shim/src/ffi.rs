@@ -25,7 +25,7 @@ pub struct dfd_exec_options {
     pub pipeline_depth: i32,
     pub pinned_pool_chunks: i32,
     pub max_pinned_chunks: i32,
-    pub reserved: i32,
+    pub device_output: i32,
 }
 
 /// `dfd_exec_stats` (include/dfd_b200.h).
@@ -55,6 +55,17 @@ pub struct ArrowDeviceArray {
     pub reserved: [i64; 3],
 }
 pub const ARROW_DEVICE_CUDA: i32 = 2;
+
+/// `struct ArrowDeviceArrayStream` of the Arrow C Device stream interface (`include/arrow_c_abi.h`).
+#[repr(C)]
+pub struct ArrowDeviceArrayStream {
+    pub device_type: i32,
+    pub get_schema: Option<unsafe extern "C" fn(*mut ArrowDeviceArrayStream, *mut FFI_ArrowSchema) -> c_int>,
+    pub get_next: Option<unsafe extern "C" fn(*mut ArrowDeviceArrayStream, *mut ArrowDeviceArray) -> c_int>,
+    pub get_last_error: Option<unsafe extern "C" fn(*mut ArrowDeviceArrayStream) -> *const c_char>,
+    pub release: Option<unsafe extern "C" fn(*mut ArrowDeviceArrayStream)>,
+    pub private_data: *mut c_void,
+}
 
 // dfd_status (include/dfd_b200.h)
 pub const DFD_OK: c_int = 0;
@@ -94,6 +105,11 @@ extern "C" {
     pub fn dfd_repartition_exec_abort(x: *mut dfd_repartition_exec, message: *const c_char) -> c_int;
     /// `plan.execute(partition, ctx)` (impl_execute_task.rs:77-86): a blocking Arrow C stream of that destination's batches.
     pub fn dfd_repartition_exec_execute(x: *mut dfd_repartition_exec, partition: u32, out: *mut FFI_ArrowArrayStream) -> c_int;
+    /// The same for an operator created with `device_output = 1`: a blocking Arrow C Device stream of GPU-resident batches,
+    /// each with a `sync_event` the consumer's stream waits on; a batch is released after the consumer's device reads.
+    pub fn dfd_repartition_exec_execute_device(x: *mut dfd_repartition_exec, partition: u32, out: *mut ArrowDeviceArrayStream) -> c_int;
+    /// Pulls a stream of GPU-resident batches to exhaustion (through `push_device`), then finishes; releases the stream once.
+    pub fn dfd_repartition_exec_run_device(x: *mut dfd_repartition_exec, input: *mut ArrowDeviceArrayStream) -> c_int;
     pub fn dfd_repartition_exec_stats(x: *mut dfd_repartition_exec, out: *mut dfd_exec_stats) -> c_int;
     pub fn dfd_repartition_exec_destroy(x: *mut dfd_repartition_exec);
 }
