@@ -17,7 +17,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT_DIR = os.path.join(HERE, "_lib")
 OBJ_DIR = os.environ.get("DFD_OBJ_DIR", os.path.join(OUT_DIR, "obj"))
 
-SOURCES = ["dfd_api.cu", "dfd_exec.cu", "dfd_exchange.cu", "dfd_reduce.cu", "dfd_stage.cu", "dfd_emit.cu", "dfd_scatter_twopass_local.cu", "dfd_scatter_twopass_peer.cu",
+SOURCES = ["dfd_api.cu", "dfd_exec.cu", "dfd_exchange.cu", "dfd_reduce.cu", "dfd_stage.cu", "dfd_emit.cu", "dfd_gather.cu", "dfd_scatter_twopass_local.cu", "dfd_scatter_twopass_peer.cu",
            "dfd_scatter_onepass_local.cu", "dfd_scatter_onepass_peer.cu", "dfd_scatter_follow_local.cu", "dfd_scatter_follow_peer.cu"]
 TUNABLE = {s for s in SOURCES if s.startswith("dfd_scatter_") or s == "dfd_api.cu"}  # sources that see the tile-geometry macros
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper); the code also needs a device of exactly this capability

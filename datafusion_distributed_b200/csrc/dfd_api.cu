@@ -140,6 +140,7 @@ int dfd::PartitionJob::prepare(Partitioner* part, const dfd_column* in_cols, int
     n_rows = rows;
     passes.clear();
     var_cols.clear();
+    gathers.clear();
     d_src = nullptr;
     bytes = 0;
     Ctx* c = p->ctx;
@@ -158,9 +159,13 @@ int dfd::PartitionJob::prepare(Partitioner* part, const dfd_column* in_cols, int
         const bool var_kind = ic.kind == DFD_COL_UTF8 || ic.kind == DFD_COL_LARGE_UTF8 || ic.kind == DFD_COL_BINARY;
         if (!var_kind && (!ic.values || (!peer && !oc.values))) return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: values is NULL", i);
         PayloadCol pc{};
-        if (ic.kind == DFD_COL_FIXED) {
-            if (ic.width != 1 && ic.width != 2 && ic.width != 4 && ic.width != 8 && ic.width != 16)
-                return set_error(DFD_ERR_UNSUPPORTED, "column %d: fixed width %d not in {1,2,4,8,16}", i, ic.width);
+        if (ic.kind == DFD_COL_FIXED && !scatter_width(ic.width)) {
+            // any other width: no alignment rule, gathered through d_src after K2 (k_gather_rows)
+            if (!gather_wide) return set_error(DFD_ERR_UNSUPPORTED, "column %d: fixed width %d not in {1,2,4,8,16}", i, ic.width);
+            if (ic.width < 1) return set_error(DFD_ERR_UNSUPPORTED, "column %d: fixed width %d < 1", i, ic.width);
+            gathers.push_back(GatherCol{ic.values, oc.values, ic.offset, ic.width});
+            bytes += (uint64_t)n_rows * ic.width;
+        } else if (ic.kind == DFD_COL_FIXED) {
             if (((uintptr_t)ic.values | (uintptr_t)oc.values) & (uintptr_t)(ic.width - 1))
                 return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: buffers must be aligned to the value width", i);
             pc.in = ic.values;
@@ -204,7 +209,7 @@ int dfd::PartitionJob::prepare(Partitioner* part, const dfd_column* in_cols, int
         } else {
             return set_error(DFD_ERR_UNSUPPORTED, "column %d: unknown column kind %d", i, ic.kind);
         }
-        if (ic.kind == DFD_COL_FIXED || ic.kind == DFD_COL_BOOL) passes.push_back(pc);
+        if ((ic.kind == DFD_COL_FIXED && scatter_width(ic.width)) || ic.kind == DFD_COL_BOOL) passes.push_back(pc);
         if (ic.validity) {
             if (peer) return set_error(DFD_ERR_UNSUPPORTED, "column %d: nullable columns need the NCCL exchange mode", i);
             if (!oc.validity) return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: input has a validity bitmap but out validity is NULL", i);
@@ -228,8 +233,8 @@ int dfd::PartitionJob::prepare(Partitioner* part, const dfd_column* in_cols, int
                 if (e != cudaSuccess) return cuda_error(e, "cudaMemsetAsync(bit-packed output)");
             }
     }
-    if (!var_cols.empty() && n_rows > 0) {
-        // K4 needs the input row of every output row: scatter an iota column with the rest
+    if ((!var_cols.empty() || !gathers.empty()) && n_rows > 0) {
+        // K4 and the gathers need the input row of every output row: scatter an iota column with the rest
         const size_t nb = (((size_t)n_rows * 4) + 255) & ~(size_t)255;
         const int64_t n_blocks = (n_rows + VAR_BLOCK * VAR_ITEMS - 1) / (VAR_BLOCK * VAR_ITEMS);
         rc = c->var_scratch.ensure(2 * nb + (size_t)(n_blocks + 1) * 8 + 256, c->device);
@@ -374,6 +379,10 @@ int dfd::PartitionJob::run_scatter(const int64_t* dest_base, void* const* peer_b
         sp.dest_cache = d_dest_cache;
         if ((rc = launch_width_groups(sp, passes, ScatterKind::TwoPass, &launches))) return rc;
     }
+    if (!gathers.empty()) {
+        int rc = run_gathers();
+        if (rc) return rc;
+    }
     if (!var_cols.empty()) {
         int rc = run_varwidth();
         if (rc) return rc;
@@ -471,6 +480,18 @@ static int launch_varwidth(const dfd::PartitionJob::VarCol& vc, const uint32_t* 
     return DFD_OK;
 }
 
+// One k_gather_rows launch per gathered column (none for 0 rows); counted as kernel launches, not scatter launches.
+int dfd::PartitionJob::run_gathers() {
+    if (n_rows == 0) return DFD_OK;
+    Ctx* c = p->ctx;
+    for (const GatherCol& g : gathers) {
+        int rc = launch_gather_rows(g.in, g.in_offset, d_src, n_rows, g.width, g.out, c->sm_count, stream);
+        if (rc) return rc;
+        c->metrics.kernel_launches++;
+    }
+    return DFD_OK;
+}
+
 int dfd::PartitionJob::run_varwidth() {
     Ctx* c = p->ctx;
     for (const VarCol& vc : var_cols) {
@@ -549,6 +570,7 @@ int dfd::partition_device_locked(Partitioner* p, const dfd_column* in_cols, int 
                                  const dfd_column* out_cols, cudaStream_t stream, bool var_bytes_known) {
     PartitionJob job;
     job.var_bytes_known = var_bytes_known;
+    job.gather_wide = true;
     int rc = job.prepare(p, in_cols, n_cols, n_rows, out_cols, false, stream);
     if (rc) return rc;
     if ((rc = job.run_hist_scan())) return rc;
@@ -989,6 +1011,8 @@ int dfd_partition_device_onepass(dfd_partitioner* p, const dfd_column* in_cols, 
     const uint32_t N = p->N;
     bool has_fixed = false, has_var = false;
     for (int i = 0; i < n_cols; ++i) {
+        if (in_cols[i].kind == DFD_COL_FIXED && !scatter_width(in_cols[i].width))
+            return set_error(DFD_ERR_UNSUPPORTED, "column %d: fixed width %d not in {1,2,4,8,16} (wide values: dfd_partition_device)", i, in_cols[i].width);
         has_fixed |= in_cols[i].kind == DFD_COL_FIXED;
         has_var |= in_cols[i].kind == DFD_COL_UTF8 || in_cols[i].kind == DFD_COL_LARGE_UTF8 || in_cols[i].kind == DFD_COL_BINARY;
     }

@@ -138,12 +138,15 @@ struct PartitionJob {
     std::vector<PayloadCol> passes;
     struct VarCol { dfd_column in, out; };
     std::vector<VarCol> var_cols;        // K4: variable-width payload columns
-    uint32_t* d_src = nullptr;            // K4: input row of every output row (scattered iota)
+    uint32_t* d_src = nullptr;            // K4 and the gathers: input row of every output row (scattered iota)
     unsigned long long* d_block_sums = nullptr;
     uint64_t bytes = 0;
     int64_t n_rows = 0, n_tiles = 0;
     bool var_bytes_known = false;        // set before prepare(): in_cols[i].values_bytes IS the byte count of a var-width input (no D2H read + sync)
     bool onepass_tiling = false;         // set before prepare(): tile the rows for the single-pass kernel (ONEPASS_K rows per thread)
+    bool gather_wide = false;            // set before prepare(): accept fixed widths outside {1,2,4,8,16} (two-pass local calls)
+    struct GatherCol { const void* in; void* out; int64_t in_offset, width; };
+    std::vector<GatherCol> gathers;      // wide fixed-width columns, gathered through d_src after K2 (k_gather_rows)
     int64_t out_rows = -1;               // rows of the OUTPUT row space (-1: n_rows; single-pass regions: N * region_rows)
     uint32_t* d_hist = nullptr;
     uint32_t* d_base = nullptr;
@@ -157,6 +160,7 @@ struct PartitionJob {
     int run_scatter(const int64_t* dest_base, void* const* peer_base, int world, uint32_t parts_per_rank,
                     const int32_t* abort_flag);
     int run_varwidth();  // called by run_scatter after the fixed-width launches
+    int run_gathers();   // called by run_scatter after the fixed-width launches
     // Single-pass K2 (no K1/K1b): destinations live in fixed regions; see k_scatter<..., ONEPASS>.
     struct OnePassLayout {
         const int64_t* d_dest_base = nullptr;  // device [N] region starts (rows); nullptr: region_stride formula
@@ -186,6 +190,12 @@ int launch_bytes_to_bits(const uint8_t* in, int64_t n, void* out_words, cudaStre
 int launch_offsets_to_lengths(const void* off, int ow, int64_t n, void* len, cudaStream_t s);
 int launch_var_dest_bytes(const void* off, int ow, const int64_t* part_starts, uint32_t N, int64_t* bytes, int64_t* first, cudaStream_t s);
 int launch_lengths_to_offsets(const void* len, int ow, int64_t n, unsigned long long* block_sums /*[n/2048 + 2]*/, void* out_off, cudaStream_t s);
+
+// Gather after K2 through src, the input row of every output row (kernel in dfd_gather.cu): out row j (w bytes) = in row
+// in_offset + src[j], for the fixed widths no scatter instantiation moves.
+int launch_gather_rows(const void* in, int64_t in_offset, const uint32_t* src, int64_t n_rows, int64_t w, void* out, int sm_count, cudaStream_t s);
+// Fixed widths the scatter instantiations move; other widths are gathered (two-pass local partition calls only).
+inline bool scatter_width(int64_t w) { return w == 1 || w == 2 || w == 4 || w == 8 || w == 16; }
 
 // Device-side chunk assembly for device-resident input batches (dfd_repartition_exec_push_device; kernels in dfd_stage.cu).
 // One StageJob appends one buffer of one column to the open chunk; all jobs of a pushed batch go out in one launch
@@ -272,6 +282,7 @@ constexpr int32_t COL_INTERVAL_DAY_TIME = 5, COL_INTERVAL_MONTH_DAY_NANO = 6;
 int hash_columns_locked(Ctx* c, const dfd_column* cols, int n_cols, int64_t n_rows, const uint64_t* seeds, uint64_t* hashes_device, cudaStream_t stream);
 
 // Launches K1 -> K1b -> K2 on `stream`; caller holds ctx->mu and has set the device.
+// Fixed-width values of any width >= 1 are accepted: widths outside {1,2,4,8,16} are gathered after K2.
 int partition_device_locked(Partitioner* p, const dfd_column* in_cols, int n_cols, int64_t n_rows,
                             const dfd_column* out_cols, cudaStream_t stream, bool var_bytes_known = false);
 

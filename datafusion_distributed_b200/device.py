@@ -184,6 +184,16 @@ class DeviceColumn:
             keep += [ob, db]
             return DeviceColumn(kind, 0, db.ptr, ob.ptr, validity, arr.offset, len(arr), keep, t,
                                 bufs[2].size if bufs[2] is not None else 0)
+        if pa.types.is_fixed_size_list(t):
+            # one FIXED column of n x (child width) bytes per row: the child's values from its first element on
+            child = arr.values
+            if child.null_count or not pa.types.is_primitive(child.type) or pa.types.is_boolean(child.type):
+                raise ValueError(f"FixedSizeList column: the child must be a non-null fixed-width primitive, not {child.type}")
+            cw = child.type.bit_width // 8
+            cb = child.buffers()[1]
+            b = ctx.upload_raw(cb.address + child.offset * cw, len(child) * cw)
+            keep.append(b)
+            return DeviceColumn(nv.COL_FIXED, t.list_size * cw, b.ptr, 0, validity, arr.offset, len(arr), keep, t)
         width = t.bit_width // 8
         b = ctx.upload_raw(bufs[1].address, bufs[1].size, pad_to=max(width, 4))
         keep.append(b)
@@ -232,7 +242,11 @@ class DeviceColumn:
         if self.kind == nv.COL_FIXED:
             raw = self.keep[-1].download(np.uint8, self.length * self.width)
             data = pa.py_buffer(raw[start * self.width: stop * self.width].tobytes())
-            return pa.Array.from_buffers(self.arrow_type, n, [validity_buf, data], null_count=null_count)
+            t = self.arrow_type
+            if t is not None and pa.types.is_fixed_size_list(t):
+                child = pa.Array.from_buffers(t.value_type, n * t.list_size, [None, data])
+                return pa.Array.from_buffers(t, n, [validity_buf], null_count=null_count, children=[child])
+            return pa.Array.from_buffers(t, n, [validity_buf, data], null_count=null_count)
         # variable width: rebase the offsets of rows [start, stop) to zero
         odt = np.int64 if self.kind == nv.COL_LARGE_UTF8 else np.int32
         off = self.keep[-2].download(odt, self.length + 1)[start:stop + 1]

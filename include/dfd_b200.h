@@ -53,7 +53,7 @@ typedef struct dfd_partitioner dfd_partitioner; /* ≙ BatchPartitioner::Hash   
 /* Physical layout of one column, device- or host-resident: the buffers of an
  * Arrow array flattened (what ArrowArray.buffers[] holds for these types). */
 typedef enum {
-    DFD_COL_FIXED = 0,     /* primitive values, `width` bytes each (1,2,4,8,16)     */
+    DFD_COL_FIXED = 0,     /* values of `width` bytes each (see dfd_column.width)   */
     DFD_COL_BOOL = 1,      /* bit-packed values                                     */
     DFD_COL_UTF8 = 2,      /* int32 offsets + bytes; hashed as Rust `str`           */
     DFD_COL_LARGE_UTF8 = 3,/* int64 offsets + bytes                                 */
@@ -62,7 +62,10 @@ typedef enum {
 
 typedef struct {
     int32_t kind;            /* dfd_col_kind                                         */
-    int32_t width;           /* DFD_COL_FIXED: bytes per value                       */
+    int32_t width;           /* DFD_COL_FIXED: bytes per value.  1/2/4/8/16 everywhere;
+                                any other width >= 1 (a FixedSizeList row, e.g. an
+                                embedding of n floats = 4n bytes) in dfd_partition_device
+                                only, as payload, with no alignment rule                */
     void* values;            /* values / bitmap / string bytes                       */
     void* offsets;           /* var-width kinds only                                 */
     uint8_t* validity;       /* Arrow validity bitmap (LSB first) or NULL = no nulls */
@@ -193,6 +196,8 @@ int dfd_partition_ids_device(dfd_partitioner* p, const dfd_column* cols, int n_c
  * `values` with `values_bytes` >= the input's byte count; the output is one
  * offsets buffer + one byte buffer in destination order, so destination p is
  * again the zero-copy slice [part_starts[p], part_starts[p+1]).
+ * Fixed-width payload columns of a width outside 1/2/4/8/16 are gathered after the scatter through
+ * the input row of every output row (k_gather_rows); keys must still be 1/2/4/8/16 bytes wide.
  * At most 2^32 - 1 rows per call; more: DFD_ERR_UNSUPPORTED, before any allocation or launch. */
 int dfd_partition_device(dfd_partitioner* p, const dfd_column* in_cols, int n_cols,
                          int64_t n_rows, const dfd_column* out_cols, int64_t* part_starts_host);
@@ -209,6 +214,7 @@ const int64_t* dfd_partitioner_part_starts_device(const dfd_partitioner* p);
  *   N * region_rows >= 2^32 - 1 is DFD_ERR_UNSUPPORTED (the largest accepted product is 2^32 - 2).
  *   If a destination outgrows its region (skewed keys) nothing is lost: collection re-runs
  *   the kernel with exact regions (part_starts = prefix sums of the now-known counts, dense).
+ *   Fixed-width columns of other than 1/2/4/8/16 bytes: DFD_ERR_UNSUPPORTED (dfd_partition_device moves them).
  *   Variable-width payload columns, boolean-only schemas and N > 256 take the two-pass
  *   path internally and return the dense layout through the same (start, count) contract.
  * part_starts_host / part_counts_host (N int64 each): both NULL = asynchronous on
