@@ -906,18 +906,26 @@ static int push_slices_locked(dfd_exchange* x, const std::vector<PushCol>& pc, c
         Lo.seg_start.assign(nseg, 0);
         Lo.bseg_start.assign(V, std::vector<int64_t>(nseg, 0));
         int64_t run = 0;
-        std::vector<int64_t> brun(V, 0);
+        std::vector<int64_t> brun(V, 0), bmax(V, 0);  // bmax: the largest string offset any segment of the column holds
         for (uint32_t sg = 0; sg < nseg; ++sg) {
             int r;
             uint32_t g;
             R.source(o, sg, &r, &g);
             Lo.seg_start[sg] = run;
-            run = (run + (r >= 0 ? rows_of(r, g) : 0) + 1 + 31) / 32 * 32;  // 32-row aligned, >= 1 spare row
+            const int64_t rows = r >= 0 ? rows_of(r, g) : 0;
+            run = (run + rows + 1 + 31) / 32 * 32;  // 32-row aligned, >= 1 spare row
             for (int v = 0; v < V; ++v) {
+                const int64_t nb = r >= 0 ? bytes_of(r, v, g) : 0;
                 Lo.bseg_start[v][sg] = brun[v];
-                brun[v] = (brun[v] + (r >= 0 ? bytes_of(r, v, g) : 0) + 15) / 16 * 16;
+                if (rows > 0) bmax[v] = brun[v] + nb;
+                brun[v] = (brun[v] + nb + 15) / 16 * 16;
             }
         }
+        // A Utf8 / Binary segment's int32 offsets index the column's one byte region, 16-byte padding included: a
+        // consumer whose offsets would pass INT32_MAX cannot take this round, exactly like one whose window is too small.
+        int narrow = -1;
+        for (int i = 0; i < n_cols && narrow < 0; ++i)
+            if (pc[i].var_index >= 0 && pc[i].ow == 4 && bmax[pc[i].var_index] > INT32_MAX) narrow = i;
         Lo.reg_values.assign(n_cols, 0); Lo.reg_off.assign(n_cols, 0); Lo.reg_valid.assign(n_cols, 0);
         size_t off = 0;
         for (int i = 0; i < n_cols; ++i) {
@@ -930,7 +938,7 @@ static int push_slices_locked(dfd_exchange* x, const std::vector<PushCol>& pc, c
             }
             if (q.nullable) { Lo.reg_valid[i] = off; off += al((size_t)run / 8 + 16); }
         }
-        if (off > x->window_bytes) {
+        if (off > x->window_bytes || narrow >= 0) {
             // Every worker takes this branch (same matrices).  Nobody may start the next exchange — and overwrite its metadata
             // slots in the peers' headers — before every worker has read THIS epoch's metadata: close the epoch with the
             // done barrier, exactly as a successful exchange does (the back-pressured stream retries at once with a finer
@@ -941,6 +949,9 @@ static int push_slices_locked(dfd_exchange* x, const std::vector<PushCol>& pc, c
             CUDA_TRY(cudaMemcpyAsync(x->h_seg_flags + MAX_RANKS, x->d_flags + 1, sizeof(int32_t), cudaMemcpyDeviceToHost, s), "D2H timeout flag");
             CUDA_TRY(cudaStreamSynchronize(s), "push exchange (capacity)");
             if (x->h_seg_flags[MAX_RANKS]) return set_error(DFD_ERR_INTERNAL, "a peer worker never acknowledged the over-full round (did it fail?)");
+            if (narrow >= 0)
+                return set_error(DFD_ERR_CAPACITY, "column %d: consumer %d would hold string offsets up to %lld, past the int32 offsets of "
+                                                   "Utf8 / Binary", narrow, o, (long long)bmax[pc[narrow].var_index]);
             return set_error(DFD_ERR_CAPACITY, "consumer %d needs %zu B of receive window for this exchange, windows hold %zu B", o, off, x->window_bytes);
         }
     }
@@ -1209,6 +1220,20 @@ int dfd_shuffle_device(dfd_exchange* x, dfd_partitioner* part, int mode, const d
     }
     cudaError_t se = cudaStreamSynchronize(s);
     if (se != cudaSuccess) return cuda_error(se, "count exchange");
+    // The receiver rebuilds a Utf8 / Binary column's int32 offsets from lengths: no consumer may receive more than INT32_MAX
+    // bytes of one.  Checked for every consumer from the all-gathered matrices, so that all workers refuse together and none
+    // is left waiting in a send to a peer that refused.
+    for (size_t v = 0; v < V; ++v) {
+        if (pc[var_cols[v]].ow != 4) continue;
+        for (int o = 0; o < T; ++o) {
+            int64_t total = 0;
+            for (int r = 0; r < T; ++r)
+                for (uint32_t q = 0; q < P; ++q) total += h_bytes[v * (size_t)T * N + (size_t)r * N + (size_t)o * P + q];
+            if (total > INT32_MAX)
+                return set_error(DFD_ERR_CAPACITY, "column %d: consumer %d would receive %lld string bytes, past the int32 offsets of Utf8 / "
+                                                   "Binary", var_cols[v], o, (long long)total);
+        }
+    }
     std::vector<int64_t> send_start(N), recv_start((size_t)P * T);
     int64_t recv_rows = 0;
     rc = dfd_exchange_plan(T, P, x->rank, x->h_counts, send_start.data(), recv_start.data(), part_starts_host, nullptr, &recv_rows);

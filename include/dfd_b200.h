@@ -451,7 +451,9 @@ int dfd_exchange_plan(int world, uint32_t partitions_per_task, int rank, const i
  *   FUSED mode: out_cols[c].values are SET to point into the receive window
  *               (valid until the next shuffle); out_capacity_rows is ignored.
  * DFD_ERR_CAPACITY if a receive buffer / window is too small (nothing is
- * written in that case). */
+ * written in that case), and in NCCL mode on every worker if any worker would
+ * receive more than INT32_MAX bytes of one Utf8 / Binary column (its int32
+ * offsets could not index them; LargeUtf8 has no such limit). */
 int dfd_shuffle_device(dfd_exchange* x, dfd_partitioner* p, int mode, const dfd_column* in_cols, int n_cols,
                        int64_t n_rows, uint32_t partitions_per_task, dfd_column* out_cols,
                        int64_t out_capacity_rows, int64_t* part_starts_host);
@@ -483,7 +485,11 @@ int dfd_exchange_wait(dfd_exchange* x, int64_t* part_starts_host);
  * segment starts on a 32-row boundary; out_cols[c].offsets / .validity are set like .values, and the string offsets
  * of a segment index the column's single `values` byte buffer directly (Arrow layout, zero-copy sliceable).  ON
  * ENTRY out_cols[c].validity != NULL marks column c as nullable in the SCHEMA (all workers must agree), whether or
- * not this worker's rows contain nulls; in_cols[c].values_bytes must hold the byte size of a string column's data. */
+ * not this worker's rows contain nulls; in_cols[c].values_bytes must hold the byte size of a string column's data.
+ * The push transport returns DFD_ERR_CAPACITY on every worker, with nothing pushed, when some consumer's window is too
+ * small or when a Utf8 / Binary column's offsets there would pass INT32_MAX: the byte region they index holds every
+ * segment's bytes, each segment's start rounded up to 16 bytes.  dfd_shuffle_stream_next then retries in smaller
+ * rounds; dfd_exchange_gather reports the same condition. */
 int dfd_shuffle_device_onepass(dfd_exchange* x, dfd_partitioner* p, const dfd_column* in_cols, int n_cols, int64_t n_rows,
                                uint32_t partitions_per_task, dfd_column* out_cols);
 int dfd_exchange_collect(dfd_exchange* x, dfd_column* out_cols, int64_t* seg_starts, int64_t* seg_counts);

@@ -4,7 +4,8 @@ push transport and compare every (partition, producer) segment with the single-n
 
     python run_workers.py <harness.so> <world> <scenario> [seed]
 
-scenario: shuffle | stream | coalesce | broadcast | mismatch | onepass | onepass_overflow | host | peer_missing | mixed | nccl | fused | stale"""
+scenario: shuffle | stream | coalesce | broadcast | mismatch | onepass | onepass_overflow | host | peer_missing | mixed | nccl | nccl_int32 | fused |
+          stale"""
 import ctypes as C
 import os
 import sys
@@ -270,6 +271,28 @@ def worker(lib, rank, world, uid, scenario, seed, errors, barrier):
             one_single_pass(seed + 3)
             one_single_pass(seed + 4)
             one_push(seed + 5)
+        elif scenario == "nccl_int32":
+            # NCCL mode, one key value: every row of both producers goes to one consumer, which would receive more than INT32_MAX
+            # bytes of a Utf8 column.  EVERY worker refuses before any send, the one that would receive nothing included.
+            rows, row_bytes = 1100, 1 << 20
+            assert world * rows * row_bytes > 2**31 - 1 >= rows * row_bytes
+            off = (np.arange(rows + 1, dtype=np.int64) * row_bytes).astype(np.int32)
+            s_big = pa.Array.from_buffers(pa.string(), rows, [None, pa.py_buffer(off.tobytes()), pa.py_buffer(np.full(rows * row_bytes, 97, np.uint8))])
+            t_big = pa.table([pa.array(np.full(rows, 7, np.int64)), s_big], names=["key", "s"])
+            kp = []
+            cols_ = to_columns(t_big, kp)
+            pt = VP()
+            check(lib, lib.dfd_partitioner_create(ctx, N, (C.c_int32 * 1)(0), 1, None, C.byref(pt)), "dfd_partitioner_create")
+            o_ = (COL * 2)()
+            small = [np.zeros(64, np.uint8) for _ in range(3)]
+            o_[0].kind, o_[0].width, o_[0].values = nv.COL_FIXED, 8, small[0].ctypes.data
+            o_[1].kind, o_[1].offsets, o_[1].values, o_[1].values_bytes = nv.COL_UTF8, small[1].ctypes.data, small[2].ctypes.data, 64
+            ps = (C.c_int64 * (P + 1))()
+            rc = lib.dfd_shuffle_device(ex, pt, 0, cols_, 2, rows, P, o_, 8, ps)
+            err = lib.dfd_last_error()
+            assert rc == 7 and b"int32" in err, (rank, rc, err)
+            barrier.wait()
+            lib.dfd_partitioner_destroy(pt)
         elif scenario == "stale":
             # collect reports the LAST shuffle only: a push result is dropped as soon as another shuffle starts, an asynchronous
             # two-pass shuffle is completed by collect in its dense layout, and after an NCCL-mode shuffle (complete inside the

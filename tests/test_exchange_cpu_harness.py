@@ -96,6 +96,11 @@ def test_nccl_mode_moves_every_column_kind(exchange_harness, world):
     run(exchange_harness, world, "nccl")
 
 
+def test_nccl_mode_refuses_int32_offsets_past_int32_max_on_every_worker(exchange_harness):
+    """Two producers of 1.1 GiB of Utf8 each, all for one consumer: DFD_ERR_CAPACITY on both workers before any send."""
+    run(exchange_harness, 2, "nccl_int32")
+
+
 @pytest.mark.parametrize("world", [1, 2, 4])
 def test_two_pass_fused_transport_dense_layout(exchange_harness, world):
     run(exchange_harness, world, "fused")
