@@ -125,7 +125,8 @@ __global__ void __launch_bounds__(256) k_group_count(const __grid_constant__ Red
 }
 
 // `rep` = the group's representative row.  Float MIN / MAX start from its value, not from +-inf: an all-NaN group then
-// yields one of its own NaNs, and folding the representative in again in k_group_combine changes nothing.
+// yields one of its own NaNs, and folding the representative in again in k_group_combine changes nothing.  Float SUM
+// starts from +0.0 (dfd_b200.h): a group of only -0.0 values sums to +0.0.
 __device__ __forceinline__ void state_init(const ReduceCol& c, char* dst, int64_t rep) {
     switch (c.op) {
         case DFD_AGG_SUM_I64: case DFD_AGG_SUM_F64: *(uint64_t*)dst = 0; break;

@@ -510,7 +510,9 @@ int dfd_exchange_phase_ms(dfd_exchange* x, double* out3, uint64_t* n_shuffles);
  * Fixed-width non-null keys and states (nullable group keys / states: DFD_ERR_UNSUPPORTED).  Synchronous.
  * At most 2^31 rows per call (the group table has up to 2^32 slots of 32-bit indices); more: DFD_ERR_UNSUPPORTED,
  * returned before anything is allocated or launched.
- * Integer SUMs wrap (two's complement, mod 2^64 / 2^128).  Float SUM is the IEEE sum in an unspecified order.  Float
+ * Integer SUMs wrap (two's complement, mod 2^64 / 2^128).  Float SUM starts from +0.0 and adds the group's values in an
+ * unspecified order, so a group whose values are all -0.0 sums to +0.0, not to their IEEE sum -0.0 (whether DataFusion's
+ * sum accumulator does the same has not been verified).  Float
  * MIN / MAX order values by IEEE 754 totalOrder (Rust's f64::total_cmp): -NaN < -inf < ... < -0.0 < +0.0 < ... < +inf
  * < +NaN, NaNs ordered by payload.  So a +NaN wins MAX and a -NaN wins MIN, -0.0 is below +0.0, an all-NaN group yields
  * one of its NaNs, and the result's bits are one input row's bits, the same on every run. */
