@@ -102,3 +102,53 @@ def test_crafted_reduce_keys_all_land_on_the_last_slot():
     for k in keys.tolist():
         assert reduce_slot_of_i64_key(k, slots) == slots - 1
         assert mix64(REDUCE_HASH_SEED ^ (k & M64)) & (slots - 1) == slots - 1
+
+
+def test_constructed_destination_runs_reach_the_slot_bounds():
+    """The single-pass layout constructions: every tile gives its intended counts under the destination table, and the
+    restated pair and slot totals reach the bounds the write-out caps are sized for.  T = 2560 (the default tiling)."""
+    from tests.util import (aligned_run_slots, keys_for_counts, onepass_run_pairs, region_construction, residue_sweep_counts,
+                            run_starts, tile_slots, worst_case_counts)
+
+    T = 2560
+    # the run restatements on hand-checked runs: o = 63, count 2 pays a 31-pair front pad, 2 pairs and a 31-pair round up
+    assert onepass_run_pairs(63, 2, 16) == 64 and onepass_run_pairs(64, 2, 16) == 32 and onepass_run_pairs(5, 0, 16) == 0
+    assert onepass_run_pairs(63, 2, 17) == 2 and onepass_run_pairs(62, 2, 17) == 1 and onepass_run_pairs(1, 3, 256) == 2
+    assert aligned_run_slots(31, 2) == 64 and aligned_run_slots(32, 2) == 32 and aligned_run_slots(7, 0) == 0
+    for N, kind in ((16, "i64"), (8, "i16"), (17, "i64"), (256, "i16")):
+        M = 64 if N <= 16 else 2
+        lut = dest_lut(kind, N)
+        for delta in (1, 0, 31, -1):
+            cnt, rr = region_construction(lambda b: worst_case_counts(N, T, 3, b), N, delta, M)
+            tot = cnt.sum(axis=0)
+            assert rr == tot.max() + delta and tot[0] == tot.max() and (tot.sum() <= rr * N)
+            assert (cnt[:-1].sum(axis=1) == T).all() and 0 < cnt[-1].sum() <= T and (cnt >= 1).all()
+            idx = keys_for_counts(cnt, lut, seed=N + delta)
+            starts = np.concatenate([[0], np.cumsum(cnt.sum(axis=1))])
+            for t in range(len(cnt)):
+                assert np.array_equal(np.bincount(lut[idx[starts[t]:starts[t + 1]]], minlength=N), cnt[t]), (N, delta, t)
+            pairs = tile_slots(cnt, np.arange(N) * rr, N)
+            rows = cnt.sum(axis=1)
+            if N == 16 and delta == 1:
+                # every run of the ragged last tile starts at 63 (mod 64) with a count of 2 (mod 64): exactly rows / 2 + 63 N
+                o = run_starts(cnt, np.arange(N) * rr)
+                assert (o[-1] % 64 == 63).all() and (cnt[-1] % 64 == 2).all()
+                assert rows[-1] == 2528 and pairs[-1] == rows[-1] // 2 + 63 * N == 2272
+            if N <= 16:
+                assert pairs.max() >= T // 2 + 63 * N - 63 and (pairs <= rows // 2 + 63 * N).all()
+            elif N == 256:
+                assert (pairs[1:] == T // 2 + N).all()  # every run odd-started with an even count
+            else:  # N = 17: full tiles keep the parity of the sum of the starts, so one run of 17 starts even
+                assert (pairs[1:-1] == T // 2 + N - 1).all()
+            assert (pairs <= (T // 2 + 63 * 16 + 255) // 256 * 256).all()  # within the KP cap of the default build
+    # the aligned write-out of a peer launch: sub-windows of 32-row multiples, full tiles reach T + 62 N less one run's pad
+    cnt = worst_case_counts(16, T, 3, [0] * 16, aligned=True)
+    slots = tile_slots(cnt, np.arange(16) * 4096, 16, aligned=True)
+    assert slots[1] == T + 62 * 16 - 32 and (slots <= T + 62 * 16).all()
+    # every run start residue mod 64, for every destination
+    for N in (3, 8):
+        cnt, rr = region_construction(lambda b: residue_sweep_counts(N, T, b, (1 - 0) % 64), N, 0, 64)
+        o = run_starts(cnt, np.arange(N) * rr) % 64
+        assert all(set(o[:, p].tolist()) == set(range(64)) for p in range(N))
+        idx = keys_for_counts(cnt, dest_lut("i64", N), seed=N)
+        assert np.array_equal(np.bincount(dest_lut("i64", N)[idx], minlength=N), cnt.sum(axis=0))

@@ -252,6 +252,184 @@ def dest_lut(kind: str, N: int) -> np.ndarray:
     return orc.partition_ids([v], len(v), N).astype(np.int32)
 
 
+# ------------------------------------------- single-pass write-out slot counts ----
+# Restatements of how many write-out slots one tile of k_scatter_onepass uses (dfd_kernels.cuh), and inputs built to use
+# as many as the tile's row count allows.  A tile holds T threads * KP (ROWS branch) or KV (aligned write-out) slots; a
+# pair or row past that cap would be dropped without a fault.
+
+PAIR_ALIGN_MAX_N = 16  # dfd_kernels.cuh: up to this N the local pairs of a run are padded to aligned 32-pair spans
+
+
+def onepass_run_pairs(o: int, cnt: int, N: int) -> int:
+    """Pairs of the run [o, o + cnt) of absolute output rows in the local single-pass write-out (the ROWS branch's `np`):
+    the run cut on even output rows, plus, for N <= PAIR_ALIGN_MAX_N, a front pad of (o >> 1) mod 32 pairs and a round up
+    to 32 pairs."""
+    if cnt == 0:
+        return 0
+    wmask = 31 if N <= PAIR_ALIGN_MAX_N else 0
+    return ((((o + cnt - 1) >> 1) - (o >> 1) + 1 + ((o >> 1) & wmask)) + wmask) & ~wmask
+
+
+def aligned_run_slots(o: int, cnt: int) -> int:
+    """Virtual slots of the run [o, o + cnt) in the aligned write-out (compute_slots with KV > K): a front pad of o mod 32
+    rows, rounded up to 32."""
+    return (o % 32 + cnt + 31) & ~31 if cnt else 0
+
+
+def run_starts(cnt: np.ndarray, base) -> np.ndarray:
+    """o[t][p] = base[p] + rows of destination p in tiles before t: the first output row of every tile's run."""
+    cnt = np.asarray(cnt, dtype=np.int64)
+    o = np.zeros_like(cnt)
+    o[1:] = np.cumsum(cnt, axis=0)[:-1]
+    return o + np.asarray(base, dtype=np.int64)[None, :]
+
+
+def tile_slots(cnt: np.ndarray, base, N: int, aligned: bool = False) -> np.ndarray:
+    """Write-out slots each tile uses: pairs (local single-pass) or aligned virtual rows."""
+    o = run_starts(cnt, base)
+    f = (lambda a, c: aligned_run_slots(a, c)) if aligned else (lambda a, c: onepass_run_pairs(a, c, N))
+    return np.array([sum(f(int(o[t, p]), int(cnt[t, p])) for p in range(N)) for t in range(len(cnt))], dtype=np.int64)
+
+
+def _slot_modulus(N: int, aligned: bool) -> int:
+    """Slots of a run depend on its start and count only modulo this (counts c and c + M differ by a whole number of
+    32-pair or 32-row spans)."""
+    return 32 if aligned else (64 if N <= PAIR_ALIGN_MAX_N else 2)
+
+
+def _best_residues(score: np.ndarray, rows: int, M: int, exact: bool):
+    """r[p] in 1..M maximising sum score[p][r - 1], with sum r <= rows and, if `exact`, sum r = rows (mod M): the rest
+    of the tile's rows then go out in whole blocks of M rows (a dynamic programme over the sum of r)."""
+    N = len(score)
+    neg = -1e18
+    dp = np.full(N * M + 1, neg)
+    dp[0] = 0.0
+    choice = np.zeros((N, N * M + 1), dtype=np.int64)
+    for p in range(N):
+        new = np.full_like(dp, neg)
+        for r in range(1, M + 1):
+            cand = np.full_like(dp, neg)
+            cand[r:] = dp[:-r] + score[p][r - 1]
+            better = cand > new
+            new[better] = cand[better]
+            choice[p][better] = r
+        dp = new
+    sums = np.arange(len(dp))
+    ok = (sums <= rows) & ((sums % M == rows % M) if exact else True)
+    s = int(np.argmax(np.where(ok, dp, neg)))
+    r = np.zeros(N, dtype=np.int64)
+    for p in reversed(range(N)):
+        r[p] = choice[p][s]
+        s -= r[p]
+    return r
+
+
+def _spread(r: np.ndarray, rows: int, M: int) -> np.ndarray:
+    """Counts r + M * k summing to `rows`: the blocks go round-robin from destination 0."""
+    blocks, N = (rows - int(r.sum())) // M, len(r)
+    assert blocks >= 0 and int(r.sum()) + blocks * M == rows
+    return r + M * (blocks // N + (np.arange(N) < blocks % N))
+
+
+def _lead_destination_0(cnt: np.ndarray, M: int, margin: int) -> np.ndarray:
+    """Move whole blocks of M rows (run-start residues unchanged) from other destinations to destination 0 until its
+    total exceeds every other by at least `margin` rows."""
+    cnt = cnt.copy()
+    while True:
+        tot = cnt.sum(axis=0)
+        q = int(np.argmax(tot[1:])) + 1 if cnt.shape[1] > 1 else 0
+        if q == 0 or tot[0] >= tot[q] + margin:
+            return cnt
+        t = int(np.argmax(cnt[:, q]))
+        assert cnt[t, q] > M, "no block left to move"
+        cnt[t, q] -= M
+        cnt[t, 0] += M
+
+
+def worst_case_counts(N: int, T: int, full_tiles: int, base, aligned: bool = False) -> np.ndarray:
+    """cnt[tile][p] for `full_tiles` tiles of T rows and a ragged last tile, built to fill the write-out slots: tiles
+    alternate between setting the run starts (as many as the row sum allows reach o = M - 1 mod M: o = 63 mod 64, a full
+    31-pair front pad and an odd start, for the local pairs at N <= 16; o odd above that; o = 31 mod 32 for the aligned
+    write-out) and spending them (counts that maximise the slots; at o = 63 that is a count = 2 mod 64, which pays the
+    full round-up too).  Tile 0 starts at `base` and always sets; the ragged last tile always spends, with as many rows
+    (<= T) as its best counts allow.  Destination 0 ends with the largest total.  Every choice is exhaustive over the
+    residues, so each tile takes the most slots its start residues and row count permit."""
+    M = _slot_modulus(N, aligned)
+    slots = (lambda o, c: aligned_run_slots(o, c)) if aligned else (lambda o, c: onepass_run_pairs(o, c, N))
+    per_row = 1.0 if aligned else 0.5
+    o = np.asarray(base, dtype=np.int64) % M
+    rows_out = []
+    for t in range(full_tiles + 1):
+        last = t == full_tiles
+        spend = last or (t > 0 and (full_tiles - t) % 2 == 0)
+        score = np.zeros((N, M))
+        for p in range(N):
+            for r in range(1, M + 1):
+                score[p][r - 1] = slots(int(o[p]) + M, r) - per_row * r  # (+ M: a start past 0, same residues)
+                if not spend:
+                    score[p][r - 1] += 1000.0 * ((o[p] + r) % M == M - 1)
+        r = _best_residues(score, T, M, exact=not last)
+        rows = T if not last else int(r.sum()) + (T - int(r.sum())) // M * M
+        rows_out.append(_spread(r, rows, M))
+        o = (o + r) % M
+    return _lead_destination_0(np.array(rows_out, dtype=np.int64), M, 2 * M)
+
+
+def residue_sweep_counts(N: int, T: int, base, end0: int, M: int = 64) -> np.ndarray:
+    """cnt[tile][p] under which every destination's run starts at every residue mod M in some tile: each full tile lets
+    all destinations but one (in turn) move to a residue they have not started at yet, the remaining one takes what the
+    row sum leaves.  A ragged last tile makes destination 0's total = end0 (mod M), and destination 0 ends with the
+    largest total."""
+    base = np.asarray(base, dtype=np.int64)
+    o, seen, rows_out = base % M, [set() for _ in range(N)], []
+    while True:
+        for p in range(N):
+            seen[p].add(int(o[p]))
+        if all(len(s) == M for s in seen) or len(rows_out) > 4 * M:
+            break
+        forced = len(rows_out) % N
+        r = np.zeros(N, dtype=np.int64)
+        for p in range(N):
+            if p != forced:
+                want = min(set(range(M)) - seen[p], default=int(o[p]) + 1)
+                r[p] = (want - o[p]) % M or M
+        r[forced] = (T - int(r.sum())) % M or M
+        rows_out.append(_spread(r, T, M))
+        o = (o + r) % M
+    r = np.ones(N, dtype=np.int64)
+    r[0] = (end0 - sum(int(c[0]) for c in rows_out)) % M or M
+    rows_out.append(_spread(r, int(r.sum()) + (T - int(r.sum())) // M * M, M))
+    return _lead_destination_0(np.array(rows_out, dtype=np.int64), M, 2 * M)
+
+
+def region_construction(make, N: int, delta: int, M: int):
+    """(cnt, region_rows) with region_rows = destination 0's total (the largest) + delta, where `make(base_residues)` builds
+    the counts against run starts p * region_rows: only region_rows mod M matters, so each residue is tried until the
+    counts it gives agree with it."""
+    tried = []
+    for r0 in sorted(range(M), key=lambda r: (r - 1 - delta) % M):  # the usual answer first: a total of 1 (mod M)
+        cnt = make([(p * r0) % M for p in range(N)])
+        rr = int(cnt[:, 0].sum()) + delta
+        if rr % M == r0:
+            return cnt, rr
+        tried.append(r0)
+    raise AssertionError(f"no consistent region size for N={N}, delta={delta}")
+
+
+def keys_for_counts(cnt: np.ndarray, dest_of_pool: np.ndarray, seed: int) -> np.ndarray:
+    """Pool indices, one per row, such that tile t holds cnt[t][p] rows whose dest_of_pool is p, shuffled within the tile
+    (so the rank of a row is not its position).  Each row is drawn at random from the pool entries of its destination."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    pools = [np.nonzero(dest_of_pool == p)[0] for p in range(cnt.shape[1])]
+    assert all(len(q) for q in pools), "a destination no key of the pool reaches"
+    out = []
+    for row in cnt:
+        tile = np.concatenate([rng.choice(pools[p], int(c)) for p, c in enumerate(row)] + [np.zeros(0, dtype=np.int64)])
+        rng.shuffle(tile)
+        out.append(tile)
+    return np.concatenate(out).astype(np.int64)
+
+
 # ---------------------------------------------- PartialReduce group hashing ----
 # Restatement of dfd_reduce.cu's key_hash for one 8-byte key, and its inverse, to craft keys that land on a chosen slot.
 
