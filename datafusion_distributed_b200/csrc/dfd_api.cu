@@ -808,8 +808,9 @@ int dfd_partitioner_create(dfd_ctx* c, uint32_t num_partitions, const int32_t* k
         return set_error(DFD_ERR_INVALID_ARGUMENT, "num_partitions %u not in [1, %u]", num_partitions, MAX_PARTITIONS);
     if (n_keys < 1 || n_keys > MAX_KEYS || !key_cols)
         return set_error(DFD_ERR_INVALID_ARGUMENT, "n_keys %d not in [1, %d]", n_keys, MAX_KEYS);
-    // worst-case shared memory of the two-pass scatter (16-byte values) must fit one CTA: fail here, not at the first launch
-    if (scatter_smem_bytes<TILE_THREADS, TILE_K>(num_partitions, 16, false, false) > 227 * 1024)
+    // worst-case shared memory of every scatter launch (16-byte values, peer, follow-up tiling) must fit one CTA: fail
+    // here, not at the first launch
+    if (scatter_smem_worst(num_partitions) > 227 * 1024)
         return set_error(DFD_ERR_UNSUPPORTED, "num_partitions %u needs more than 227 KB of shared memory per CTA", num_partitions);
     for (int k = 0; k < n_keys; ++k)
         if (key_cols[k] < 0) return set_error(DFD_ERR_INVALID_ARGUMENT, "key_cols[%d] is negative", k);

@@ -442,22 +442,25 @@ __device__ __forceinline__ int64_t region_base_of(const ScatterParams& P, uint32
 // start on a 32-row (256 B for 8-byte values) boundary of the OUTPUT buffer —
 // full-line stores to HBM and full-size write packets over NVLink.
 struct ScatterSmem {
-    // layout: stage | delta[N] | warp_cnt[W][N] | tile_start[2][N+1] | scan scratch | misc[4] | pos16[2][T] | dest8[2][T] | out_base[N] | vstart[N+1]
+    // layout: stage | delta[N] | warp_cnt[W][N] | tile_start[2][N+1] | scan scratch | misc[4] | pos16[2][T] | dest8[2][T] | vstart[N+1]
+    // out_base[N] (peer mode) reuses warp_cnt: the counters are dead once every row's staging position is known, and a
+    // 4096-destination peer launch of 16-byte values would not fit 227 KiB with a table of its own
     uint32_t off_delta, off_wc, off_ts, off_scan, off_misc, off_pos, off_d8, off_ob, off_vs;
 };
 template <int THREADS, int K>
 __host__ __device__ __forceinline__ ScatterSmem scatter_smem_layout(uint32_t N, uint32_t stage_width, bool onepass) {
     constexpr uint32_t T = THREADS * K, W = THREADS / 32;
+    static_assert(W * 4u >= 8u, "out_base[N] (8 B each) must fit in warp_cnt[W][N] (4 B each)");
     ScatterSmem L;
     L.off_delta = (T * stage_width + 15u) & ~15u;
-    L.off_wc = L.off_delta + N * 8u;
+    L.off_wc = L.off_delta + N * 8u;                                       // (8-byte aligned: off_delta is 16-byte aligned)
+    L.off_ob = L.off_wc;                                                   // peer mode only: per-destination bases
     L.off_ts = L.off_wc + W * N * 4u;
     L.off_scan = L.off_ts + (onepass ? 2u : 1u) * (N + 1u) * 4u;
     L.off_misc = L.off_scan + (W + 1u) * 4u;
     L.off_pos = (L.off_misc + 4u * 4u + 3u) & ~3u;
     L.off_d8 = L.off_pos + (onepass ? 2u * T * 2u : 0u);                  // single-pass mode: destination of every staging slot
-    L.off_ob = (L.off_d8 + (onepass ? 2u * T : 0u) + 7u) & ~7u;            // peer mode only: per-destination bases
-    L.off_vs = L.off_ob + N * 8u;                                          // aligned mode only: virtual run starts
+    L.off_vs = (L.off_d8 + (onepass ? 2u * T : 0u) + 3u) & ~3u;            // aligned mode only: virtual run starts
     return L;
 }
 
@@ -1370,7 +1373,7 @@ __global__ void __launch_bounds__(256) k_var_copy_bytes(const OFF* __restrict__ 
     }
 }
 
-// (the peer / aligned tables are last in scatter_smem_layout, so launches that do not use them do not allocate them)
+// (the aligned table is last in scatter_smem_layout, so launches that do not use it do not allocate it)
 // ---------------------------------------------------------------------------
 // Exchange helpers for bit-packed and variable-width columns (NCCL mode): bitmaps travel as one
 // byte per row, strings as (lengths, bytes); the receiver rebuilds bitmaps and offsets.
@@ -1448,10 +1451,10 @@ __global__ void __launch_bounds__(VAR_BLOCK) k_len_write_offsets(const OFF* __re
 
 template <int THREADS, int K>
 inline size_t scatter_smem_bytes(uint32_t N, int stage_width, bool peer, bool aligned, bool onepass = false) {
+    (void)peer;  // (the peer-mode output bases live in warp_cnt: a peer launch needs no more than a local one)
     const ScatterSmem L = scatter_smem_layout<THREADS, K>(N, (uint32_t)stage_width, onepass);
-    size_t off = L.off_ob;
-    if (peer || aligned) off += (size_t)N * 8;  // per-destination output bases (peer mode)
-    if (aligned) off += (size_t)(N + 1) * 4;    // virtual run starts (aligned mode)
+    size_t off = L.off_vs;
+    if (aligned) off += (size_t)(N + 1) * 4;  // virtual run starts (aligned mode)
     return off;
 }
 

@@ -60,6 +60,27 @@ constexpr int TILE_ROWS = TILE_THREADS * TILE_K;
 constexpr int ONEPASS_KV = ONEPASS_K + (62 * (int)ALIGNED_MAX_N + TILE_THREADS - 1) / TILE_THREADS;
 constexpr int ONEPASS_ROWS = TILE_THREADS * ONEPASS_K;
 
+// The most dynamic shared memory any scatter launch of a partitioner with N destinations can ask for: two-pass launches
+// of every staged width (1 B also stands for bit columns), follow-up and single-pass launches where single-pass calls
+// exist (N <= ONEPASS_MAX_N), local and peer, with the aligned write-out wherever use_aligned can turn it on (N <=
+// ALIGNED_MAX_N; DFD_ALIGNED_WRITEOUT=1 turns it on for local launches too).  dfd_partitioner_create refuses an N for
+// which this exceeds 227 KiB, so no launch of an accepted partitioner fails for lack of shared memory.
+inline size_t scatter_smem_worst(uint32_t N) {
+    size_t worst = 0;
+    const auto keep = [&worst](size_t b) { worst = b > worst ? b : worst; };
+    for (const bool peer : {false, true}) {
+        for (const bool aligned : {false, true}) {
+            if (aligned && N > ALIGNED_MAX_N) continue;
+            for (const int width : {1, 2, 4, 8, 16}) {
+                keep(scatter_smem_bytes<TILE_THREADS, TILE_K>(N, width, peer, aligned));
+                if (N > ONEPASS_MAX_N) continue;
+                keep(scatter_smem_bytes<TILE_THREADS, ONEPASS_K>(N, width, peer, aligned));
+                if (width <= 8) keep(onepass_smem_bytes<TILE_THREADS, ONEPASS_K, ONEPASS_NB, ONEPASS_SPLIT>(N, width, peer, aligned));
+            }
+        }
+    }
+    return worst;
+}
 
 // KIND picks the kernel and its tiling (see ScatterKind), V the element type, ALIGNED the write-out.  The dynamic shared
 // memory of every kind is sized and checked here.
