@@ -105,15 +105,6 @@ static int build_keyset(const dfd_partitioner* p, const dfd_column* cols, int n_
     return DFD_OK;
 }
 
-// Aligned write-out gives NVLink peer stores full-size write packets, so it is on for the fused exchange only.
-// A local single-pass launch aligns its stores without it (its KV == K write-out stores warp-aligned output-row
-// pairs, see k_scatter_onepass).  DFD_ALIGNED_WRITEOUT=0/1 forces it.
-bool dfd::use_aligned(uint32_t N, bool peer) {
-    static const int forced = [] { const char* e = getenv("DFD_ALIGNED_WRITEOUT"); return e ? (atoi(e) != 0 ? 1 : 0) : -1; }();
-    if (N > ALIGNED_MAX_N) return false;
-    return forced >= 0 ? forced == 1 : peer;
-}
-
 template <ScatterKind KIND>
 static int launch_scatter_kind(bool peer, const ScatterParams& sp, int width, bool fast, int sm_count, cudaStream_t stream) {
     return peer ? launch_scatter_impl<true, KIND>(sp, width, fast, sm_count, stream)

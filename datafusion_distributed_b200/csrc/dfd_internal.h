@@ -260,8 +260,6 @@ struct EmitJob {
 // fails with DFD_ERR_UNSUPPORTED.  libdfd_b200.so always links it.
 __attribute__((weak)) int launch_emit_chunk(const EmitJob* jobs, int n_jobs, cudaStream_t s);
 
-// Aligned write-out (k_scatter KV > K) is used for the peer-store exchange at small N (full-size NVLink write packets).
-bool use_aligned(uint32_t N, bool peer);
 // One scatter launch of a width group (template in dfd_launch.cuh).  Each (PEER, KIND) is instantiated in a translation unit
 // of its own (dfd_scatter_<kind>_<local|peer>.cu) so that they compile in parallel; nowhere else.
 template <bool PEER, ScatterKind KIND>

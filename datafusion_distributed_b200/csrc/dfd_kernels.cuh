@@ -799,6 +799,7 @@ __global__ void __launch_bounds__(THREADS + 32, MIN_CTAS) k_scatter_onepass(cons
     constexpr int BAR = 1;  // named barrier of the consumer warps
     constexpr bool ROWS = (KV == K) && !PEER;
     static_assert(!std::is_same<V, BitColumn>::value, "bit columns take the two-pass kernel");
+    static_assert(PEER || KV == K, "a local launch always takes the row-pair write-out (use_aligned, dfd_launch.cuh)");
     static_assert(NB > S, "phase 1 holds the S header items of a tile while the ring must still advance");
     static_assert(W % S == 0, "each consumer warp's rows must lie in one header item");
     constexpr int HROWS = T / S;  // rows of one header item

@@ -52,9 +52,13 @@ constexpr int ONEPASS_CTAS_PER_SM = DFD_ONEPASS_CTAS_PER_SM;
 constexpr int TILE_THREADS = DFD_TILE_THREADS;
 constexpr int TILE_K = DFD_TILE_K;
 constexpr int TILE_MIN_CTAS = DFD_TILE_MIN_CTAS;
-// aligned write-out (see k_scatter): used when N <= ALIGNED_MAX_N; each run wastes < 62 virtual slots
+// aligned write-out (see k_scatter and use_aligned): up to ALIGNED_MAX_N destinations; each run wastes < 62 virtual slots
 constexpr uint32_t ALIGNED_MAX_N = 16;
 static_assert(ALIGNED_MAX_N == PAIR_ALIGN_MAX_N, "the single-pass local write-out aligns warps for the same N");
+// The aligned write-out gives NVLink peer stores full-size write packets, so only peer launches take it.  A local
+// single-pass launch aligns its stores without it (its KV == K write-out stores warp-aligned output-row pairs, see
+// k_scatter_onepass).
+constexpr bool use_aligned(uint32_t N, bool peer) { return peer && N <= ALIGNED_MAX_N; }
 constexpr int TILE_KV = TILE_K + (62 * (int)ALIGNED_MAX_N + TILE_THREADS - 1) / TILE_THREADS;
 constexpr int TILE_ROWS = TILE_THREADS * TILE_K;
 constexpr int ONEPASS_KV = ONEPASS_K + (62 * (int)ALIGNED_MAX_N + TILE_THREADS - 1) / TILE_THREADS;
@@ -62,15 +66,15 @@ constexpr int ONEPASS_ROWS = TILE_THREADS * ONEPASS_K;
 
 // The most dynamic shared memory any scatter launch of a partitioner with N destinations can ask for: two-pass launches
 // of every staged width (1 B also stands for bit columns), follow-up and single-pass launches where single-pass calls
-// exist (N <= ONEPASS_MAX_N), local and peer, with the aligned write-out wherever use_aligned can turn it on (N <=
-// ALIGNED_MAX_N; DFD_ALIGNED_WRITEOUT=1 turns it on for local launches too).  dfd_partitioner_create refuses an N for
-// which this exceeds 227 KiB, so no launch of an accepted partitioner fails for lack of shared memory.
+// exist (N <= ONEPASS_MAX_N), local and peer, and for peer launches also with the aligned write-out wherever use_aligned
+// turns it on (N <= ALIGNED_MAX_N).  dfd_partitioner_create refuses an N for which this exceeds 227 KiB, so no launch of
+// an accepted partitioner fails for lack of shared memory.
 inline size_t scatter_smem_worst(uint32_t N) {
     size_t worst = 0;
     const auto keep = [&worst](size_t b) { worst = b > worst ? b : worst; };
     for (const bool peer : {false, true}) {
         for (const bool aligned : {false, true}) {
-            if (aligned && N > ALIGNED_MAX_N) continue;
+            if (aligned && !use_aligned(N, peer)) continue;
             for (const int width : {1, 2, 4, 8, 16}) {
                 keep(scatter_smem_bytes<TILE_THREADS, TILE_K>(N, width, peer, aligned));
                 if (N > ONEPASS_MAX_N) continue;
@@ -138,7 +142,9 @@ static int launch_scatter_kv(const ScatterParams& sp, int sm_count, cudaStream_t
 
 template <bool FAST, typename V, bool PEER, ScatterKind KIND>
 static int launch_scatter_t(const ScatterParams& sp, int sm_count, cudaStream_t stream) {
-    if (use_aligned(sp.N, PEER)) return launch_scatter_kv<FAST, V, PEER, true, KIND>(sp, sm_count, stream);
+    if constexpr (PEER) {  // (so local launches compile no aligned instantiation)
+        if (use_aligned(sp.N, PEER)) return launch_scatter_kv<FAST, V, PEER, true, KIND>(sp, sm_count, stream);
+    }
     return launch_scatter_kv<FAST, V, PEER, false, KIND>(sp, sm_count, stream);
 }
 

@@ -44,20 +44,17 @@ def test_library_is_sm90a_and_has_the_kernels(built):
     assert "VOTE" in sass  # warp-ballot ranking is in the scatter kernel
 
 
-def test_every_compiled_scatter_instantiation_is_reachable(built):
+def test_compiled_scatter_instantiations_are_exactly_the_reachable_ones(built):
     """Every scatter instantiation in the library is one the dispatch launches for some input (tests/util.py
-    scatter_dispatch), or one only an environment override reaches, each with its reason; and every reachable one is
-    compiled.  tests/test_instantiations_gpu.py launches each of them."""
+    scatter_dispatch), and every reachable one is compiled.  tests/test_instantiations_gpu.py launches each of them."""
     from datafusion_distributed_b200 import LIB_PATH
     from tests.util import compiled_scatter_instances, scatter_dispatch
 
     compiled = compiled_scatter_instances(LIB_PATH)
-    reach, env_only = scatter_dispatch()
-    assert not set(reach) & set(env_only)
-    assert all(why.startswith("env-only: ") for why in env_only.values())
-    assert sorted(compiled - set(reach) - set(env_only)) == [], "compiled, but no input launches them"
-    assert sorted(set(reach) - compiled) == [] and sorted(set(env_only) - compiled) == []
-    assert len(reach) == 79 and len(env_only) == 29  # (a change of the dispatch must revisit the GPU module's cases)
+    reach = scatter_dispatch()
+    assert sorted(compiled - set(reach)) == [], "compiled, but no input launches them"
+    assert sorted(set(reach) - compiled) == []
+    assert len(reach) == 79  # (a change of the dispatch must revisit the GPU module's cases)
 
 
 def test_header_compiles_as_plain_c(tmp_path):

@@ -1,13 +1,10 @@
 """GPU parity tests that launch every scatter instantiation the dispatch reaches (tests/util.py scatter_dispatch), one
 group of template arguments per case: narrow single-pass rings, generic keys in peer mode, peer follow-up launches, the
-two-pass fused exchange with every element width, and the local aligned write-out (in a child process that sets
-DFD_ALIGNED_WRITEOUT=1).  Each case records the kernels it launched with torch.profiler and asserts that the
-instantiations it targets ran, so a case routed elsewhere (push transport, dense fallback, another ring width) fails.
+two-pass fused exchange with every element width.  Each case records the kernels it launched with torch.profiler and
+asserts that the instantiations it targets ran, so a case routed elsewhere (push transport, dense fallback, another ring
+width) fails.
 The last test checks that the cases together launched every reachable instantiation.
 Bar: bit-exact against the oracle per destination or per segment, including row order."""
-import json
-import os
-import subprocess
 import sys
 import uuid
 
@@ -19,14 +16,11 @@ import datafusion_distributed_b200 as dfd
 from datafusion_distributed_b200 import _native as nv
 from oracle import oracle as orc
 from tests.test_onepass_gpu import check_against_oracle, dev_cols
-from tests.util import (WIDTH_V, ScatterInst, edge_sizes, expected_partitions, multi_tile_rows, scatter_dispatch, scatter_inst,
-                        scatter_instances, tile_geometry, use_aligned)
+from tests.util import (WIDTH_V, edge_sizes, expected_partitions, multi_tile_rows, scatter_dispatch, scatter_inst, scatter_instances,
+                        tile_geometry, use_aligned)
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LAUNCHED = set()  # the scatter instantiations the cases of this process ran
-CHILD_LAUNCHED = set()  # ... and those of the DFD_ALIGNED_WRITEOUT=1 child process
-LAUNCHED_JSON = "DFD_TEST_LAUNCHED_JSON"  # where a child process reports LAUNCHED
 
 SIZES = ["multi_tile", "tile_edge"]
 PS = [pytest.param(8, id="P8"), pytest.param(17, id="P17")]  # aligned / linear write-out of peer launches (ALIGNED_MAX_N = 16)
@@ -38,14 +32,6 @@ def n_rows(size):
     n = 2 * tile_geometry()[1] + 1  # two single-pass tiles and one row: a ragged two-pass tile too
     assert n in edge_sizes()
     return n
-
-
-@pytest.fixture(scope="module", autouse=True)
-def report_launched():
-    yield
-    if os.environ.get(LAUNCHED_JSON):
-        with open(os.environ[LAUNCHED_JSON], "w") as f:
-            json.dump(sorted(LAUNCHED), f)
 
 
 def profiled(fn):
@@ -255,31 +241,13 @@ def test_exchange_onepass_overflow_reruns_narrow_schema(ctx, size, P):
     assert_ran(ran, targets(1, False, [2], True, P) | targets(0, False, [2, 1], True, P))
 
 
-# --------------------------------------------------------------------------------------- aligned local write-out ----
-
-def test_local_aligned_writeout_in_child_process(tmp_path):
-    """The library reads DFD_ALIGNED_WRITEOUT once per process, so the local cases at N <= 16 run again in a child
-    pytest with DFD_ALIGNED_WRITEOUT=1: two-pass, single-pass and follow-up launches with the aligned write-out, Boolean
-    and validity columns included.  The child reports the instantiations it ran."""
-    out = tmp_path / "launched.json"
-    env = dict(os.environ, DFD_ALIGNED_WRITEOUT="1", **{LAUNCHED_JSON: str(out)})
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [
-        "-m", "pytest", os.path.abspath(__file__), "-q", "-p", "no:cacheprovider", "-k", "test_local_ and not P17 and not child_process"]
-    r = subprocess.run(cmd, cwd=ROOT, env=env, capture_output=True, text=True, timeout=1200)
-    assert r.returncode == 0, r.stdout[-4000:] + r.stderr[-4000:]
-    ran = {ScatterInst(*t) for t in json.loads(out.read_text())}
-    CHILD_LAUNCHED.update(ran)
-    _, env_only = scatter_dispatch()
-    assert set(env_only) <= ran, sorted(set(env_only) - ran)
-
-
-def test_every_reachable_instantiation_ran(request):
-    """The cases above, with the child process, launched every instantiation the dispatch reaches."""
+def test_all_reachable_instantiations_ran_in_process(request):
+    """The cases above launched every instantiation the dispatch reaches."""
     here = sys.modules[__name__]
     selected = {it.originalname for it in request.session.items if getattr(it, "module", None) is here}
     everything = {name for name in dir(here) if name.startswith("test_")}
     if selected != everything:
         pytest.skip("needs every test of the module in one run")
-    reach, env_only = scatter_dispatch()
-    missing = (set(reach) | set(env_only)) - LAUNCHED - CHILD_LAUNCHED
-    assert not missing, "never launched:\n" + "\n".join(f"{i}: {(reach | env_only)[i]}" for i in sorted(missing))
+    reach = scatter_dispatch()
+    missing = set(reach) - LAUNCHED
+    assert not missing, "never launched:\n" + "\n".join(f"{i}: {reach[i]}" for i in sorted(missing))

@@ -19,11 +19,7 @@ destinations' rows are 0 (the library zeroes bitmaps) and fixed-width rows outsi
 N * region_rows is untouched.  After a re-run, rows and bits in [n, N * region_rows) are unspecified: the first launch
 may have written there, so nothing is asserted on them.
 
-The local cases at N <= 16 run again in a child pytest under DFD_ALIGNED_WRITEOUT=1 (the aligned write-out of a local
-launch); the peer side runs the constructions through shuffle_onepass and EXCHANGE_FUSED at world 1."""
-import os
-import subprocess
-import sys
+The peer side runs the constructions through shuffle_onepass and EXCHANGE_FUSED at world 1."""
 import uuid
 
 import numpy as np
@@ -38,7 +34,6 @@ from tests.util import (PAIR_ALIGN_MAX_N, dest_lut, domain_values, expected_part
                         region_construction, residue_sweep_counts, tile_geometry, tile_slots, worst_case_counts)
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GUARD = 0xA5  # fill of every output buffer before a call
 TAIL = 64  # guard rows (and guard bitmap words) past N * region_rows
 MAX_COLS_PER_LAUNCH = 24  # dfd_types.cuh
@@ -354,18 +349,3 @@ def test_dense_fallbacks_keep_start_count_contract(ctx, n):
     run_dense(ctx, [_col(rng, "i32", n, False), strs, _col(rng, "bool", n, True), _col(rng, "i16", n, True)], [0], 17, n)
     run_dense(ctx, [_col(rng, "i64", n, False), _col(rng, "u8", n, True), _col(rng, "bool", n, True)], [0], 300, n)
 
-
-# --------------------------------------------------------------------------------------- aligned local write-out ----
-
-def test_local_layouts_aligned_writeout_in_child_process():
-    """The library reads DFD_ALIGNED_WRITEOUT once per process: the local cases at N <= 16 run again in a child pytest
-    with it set, so the local launches take the aligned write-out (KV > K)."""
-    if os.environ.get("DFD_ALIGNED_WRITEOUT"):
-        pytest.skip("already the child")
-    env = dict(os.environ, DFD_ALIGNED_WRITEOUT="1")
-    sel = "(test_local_constructed or test_local_random) and not N17 and not N48 and not N256 and not pairs17 and not pairs256"
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [
-        "-m", "pytest", os.path.abspath(__file__), "-q", "-p", "no:cacheprovider", "-k", sel]
-    r = subprocess.run(cmd, cwd=ROOT, env=env, capture_output=True, text=True, timeout=1800)
-    assert r.returncode == 0, r.stdout[-4000:] + r.stderr[-4000:]
-    assert " passed" in r.stdout, r.stdout[-2000:]

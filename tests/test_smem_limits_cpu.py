@@ -7,8 +7,7 @@ launch_scatter_kv can make for each N in [1, DFD_MAX_PARTITIONS]:
   (no bit columns in peer mode);
 - follow-up k_scatter on the single-pass tiling, and k_scatter_onepass (rings of 1-8 bytes), where single-pass calls
   exist (N <= ONEPASS_MAX_N);
-- each also with the aligned write-out where use_aligned can turn it on (N <= ALIGNED_MAX_N: peer launches, or local
-  ones under DFD_ALIGNED_WRITEOUT=1).
+- each also with the aligned write-out, which only peer launches take, where use_aligned turns it on (N <= ALIGNED_MAX_N).
 Every launch must fit, since dfd_partitioner_create accepts every such N and a launch that does not fit fails only after
 the histogram pass (and, in the exchange, after the counts were all-gathered).  The admission check (scatter_smem_worst)
 must be the largest of them."""
@@ -58,7 +57,7 @@ int main() {
 def launch_reachable(kind, width, peer, aligned, N, onepass_max_n, aligned_max_n):
     """Whether the library can make this launch for a partitioner with N destinations (the dispatch of dfd_api.cu and
     dfd_launch.cuh, as tests/util.py scatter_dispatch restates it)."""
-    if aligned and N > aligned_max_n:
+    if aligned and (not peer or N > aligned_max_n):  # use_aligned
         return False
     if peer and width == 0:  # bit columns exist only in local calls
         return False

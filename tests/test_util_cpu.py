@@ -37,8 +37,7 @@ def test_scatter_kernel_names_parse_in_every_demangler_format():
     assert scatter_inst(1, True, "u32", True, True, {}) == want
     assert scatter_inst(0, False, "bit", False, True, {}) == ScatterInst("k_scatter", 6, 10, False, "bit", False)
     assert scatter_inst(2, False, "u8", True, True, {}) == ScatterInst("k_scatter", 10, 14, False, "u8", True)
-    assert use_aligned(16, True, {}) and not use_aligned(17, True, {}) and not use_aligned(8, False, {})
-    assert use_aligned(8, False, {"DFD_ALIGNED_WRITEOUT": "1"}) and not use_aligned(8, True, {"DFD_ALIGNED_WRITEOUT": "0"})
+    assert use_aligned(16, True) and not use_aligned(17, True) and not use_aligned(8, False)
 
 
 def test_mix64_matches_the_murmur_finaliser_and_inverts():

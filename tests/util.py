@@ -157,14 +157,9 @@ def scatter_inst(mode: int, fast: bool, V: str, peer: bool, aligned: bool, env=N
     return ScatterInst("k_scatter_onepass" if mode == 1 else "k_scatter", K, KV, bool(fast), V, bool(peer))
 
 
-def use_aligned(N: int, peer: bool, env=None) -> bool:
-    """dfd::use_aligned (dfd_api.cu): the aligned write-out runs up to ALIGNED_MAX_N destinations, for peer launches only unless
-    DFD_ALIGNED_WRITEOUT=0/1 forces it (read once per process by the library)."""
-    env = os.environ if env is None else env
-    if N > _launch_defines(env)["ALIGNED_MAX_N"]:
-        return False
-    forced = env.get("DFD_ALIGNED_WRITEOUT")
-    return int(forced) != 0 if forced is not None else peer
+def use_aligned(N: int, peer: bool) -> bool:
+    """dfd::use_aligned (dfd_launch.cuh): the aligned write-out runs for peer launches of up to ALIGNED_MAX_N destinations."""
+    return peer and N <= _launch_defines({})["ALIGNED_MAX_N"]
 
 
 _ROUTES = {(0, False): "dfd_partition_device, and the local partition of the NCCL mode and the push transport (dfd_exchange.cu)",
@@ -174,13 +169,11 @@ _ROUTES = {(0, False): "dfd_partition_device, and the local partition of the NCC
            (1, True): "dfd_shuffle_device_onepass with fixed-width non-null columns (onepass_supported, dfd_exchange.cu)",
            (2, False): "dfd_partition_device_onepass: bit columns, or fixed-width columns past the first MAX_COLS_PER_LAUNCH",
            (2, True): "dfd_shuffle_device_onepass: fixed-width columns past the first MAX_COLS_PER_LAUNCH"}
-ALIGNED_LOCAL_REASON = "env-only: DFD_ALIGNED_WRITEOUT=1 (use_aligned, dfd_api.cu) is what turns on the aligned write-out of a local launch"
 
 
 def scatter_dispatch(env=None):
     """Restatement of the scatter dispatch of dfd_api.cu (PartitionJob::run_scatter, run_onepass) and dfd_launch.cuh.
-    Returns ({instantiation: route} for every instantiation an input reaches, {instantiation: reason} for those reached
-    only under an environment override).  The rules:
+    Returns {instantiation: route} for every instantiation an input reaches.  The rules:
     - widths: two-pass and follow-up launches go out one group per column width {8, 4, 16, 2, 1, 0 = bit columns}
       (PartitionJob::launch_width_groups), each mapped to V by launch_scatter_w;
     - bit columns (Boolean values, validity bitmaps) exist only in local calls: peer calls reject them
@@ -192,9 +185,9 @@ def scatter_dispatch(env=None):
       whenever the key is fast_i64 (launch_width_groups);
     - follow-up launches (mode 2, ScatterKind::FollowUp) move the bit columns and the fixed-width columns past the first
       launch (run_onepass);
-    - ALIGNED = use_aligned(N, PEER) (launch_scatter_t): for peer launches N <= 16 and N > 16 both occur; a local
-      launch is aligned only under DFD_ALIGNED_WRITEOUT=1."""
-    reach, env_only = {}, {}
+    - ALIGNED = use_aligned(N, PEER) (launch_scatter_t): ALIGNED only for peer launches at N <= 16 (peer launches occur
+      on both sides of that bound)."""
+    reach = {}
     for mode in (0, 1, 2):
         for width, V in WIDTH_V.items():
             if mode == 1 and width not in (1, 2, 4, 8):
@@ -205,14 +198,11 @@ def scatter_dispatch(env=None):
                 for fast in (False, True):
                     if mode == 1 and fast and width != 8:
                         continue
-                    for aligned in (False, True):
-                        inst = scatter_inst(mode, fast, V, peer, aligned, env)
-                        if aligned and not peer:
-                            env_only[inst] = ALIGNED_LOCAL_REASON
-                        else:
-                            reach[inst] = f"{_ROUTES[mode, peer]}; V = {V}, {'Int64 fast key' if fast else 'generic key'}" + (
-                                f", N {'<=' if aligned else '>'} 16" if peer else "")
-    return reach, env_only
+                    for aligned in ((False, True) if peer else (False,)):
+                        reach[scatter_inst(mode, fast, V, peer, aligned, env)] = (
+                            f"{_ROUTES[mode, peer]}; V = {V}, {'Int64 fast key' if fast else 'generic key'}" +
+                            (f", N {'<=' if aligned else '>'} 16" if peer else ""))
+    return reach
 
 
 # ------------------------------------------------ 32-bit limits of the ABI ----
