@@ -12,11 +12,11 @@ from .device import DeviceBuffer, DeviceColumn, WorkerContext
 from .execution_plans import PinnedTable, RepartitionExec
 from .network_shuffle import (DistributedTaskContext, ExecutionTask, NetworkBroadcastExec, NetworkCoalesceExec, NetworkShuffleExec,
                               ShuffleExchange, Stage, exchange_plan, nccl_unique_id, task_group)
-from .partitioner import HashPartitioner, PartialReduceExec, Partitioning, scale_partitioning
+from .partitioner import HashPartitioner, PartialReduceExec, Partitioning, agg_op, scale_partitioning
 
 __all__ = [
     "DfdError", "LIB_PATH", "DeviceBuffer", "DeviceColumn", "WorkerContext",
-    "HashPartitioner", "PartialReduceExec", "Partitioning", "scale_partitioning", "RepartitionExec", "PinnedTable",
+    "HashPartitioner", "PartialReduceExec", "Partitioning", "agg_op", "scale_partitioning", "RepartitionExec", "PinnedTable",
     "DistributedTaskContext", "ExecutionTask", "NetworkShuffleExec", "ShuffleExchange", "Stage", "exchange_plan", "nccl_unique_id",
     "NetworkCoalesceExec", "NetworkBroadcastExec", "task_group",
 ]

@@ -24,6 +24,9 @@ COL_FIXED, COL_BOOL, COL_UTF8, COL_LARGE_UTF8, COL_BINARY = 0, 1, 2, 3, 4
 EXCHANGE_NCCL, EXCHANGE_FUSED = 0, 1
 ROUTE_SHUFFLE, ROUTE_COALESCE, ROUTE_BROADCAST = 0, 1, 2
 AGG_SUM_I64, AGG_SUM_F64, AGG_MIN_I64, AGG_MAX_I64, AGG_SUM_I128, AGG_MIN_F64, AGG_MAX_F64 = 0, 1, 2, 3, 4, 5, 6
+AGG_MIN_I32, AGG_MAX_I32, AGG_MIN_I16, AGG_MAX_I16, AGG_MIN_I8, AGG_MAX_I8 = 7, 8, 9, 10, 11, 12
+AGG_MIN_U64, AGG_MAX_U64, AGG_MIN_U32, AGG_MAX_U32, AGG_MIN_U16, AGG_MAX_U16, AGG_MIN_U8, AGG_MAX_U8 = 13, 14, 15, 16, 17, 18, 19, 20
+AGG_MIN_I128, AGG_MAX_I128, AGG_MIN_F32, AGG_MAX_F32, AGG_MIN_F16, AGG_MAX_F16 = 21, 22, 23, 24, 25, 26
 KEY_HASH_PLAIN, KEY_HASH_INTERVAL_DAY_TIME, KEY_HASH_INTERVAL_MONTH_DAY_NANO = 0, 1, 2
 
 

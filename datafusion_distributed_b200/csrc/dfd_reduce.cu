@@ -11,7 +11,9 @@
 //   k_group_count    groups per destination partition (representatives only)      -> exclusive scan (host, N+1 values)
 //   k_group_place    every group gets an output row inside its partition; key columns copied, states initialised
 //   k_group_combine  every input row folds its states into its group's output row with atomics
-//                    (SUM i64 / f64 / i128 (two 64-bit adds with carry), MIN / MAX i64, MIN / MAX f64 under totalOrder)
+//                    (SUM i64 / f64 / i128 (two 64-bit adds with carry); MIN / MAX of signed and unsigned 8- to 64-bit
+//                    integers, of 128-bit decimals and of f16 / f32 / f64 under totalOrder: native atomicMin / atomicMax
+//                    at 32 and 64 bits, CAS loops at 8 (on the enclosing 32-bit word), 16 and 128 bits and for floats)
 // Integer / byte work; random access into an L2-resident table for the cardinalities PartialReduce is used for.
 #include <cuda_runtime.h>
 
@@ -125,8 +127,9 @@ __global__ void __launch_bounds__(256) k_group_count(const __grid_constant__ Red
 }
 
 // `rep` = the group's representative row.  Float MIN / MAX start from its value, not from +-inf: an all-NaN group then
-// yields one of its own NaNs, and folding the representative in again in k_group_combine changes nothing.  Float SUM
-// starts from +0.0 (dfd_b200.h): a group of only -0.0 values sums to +0.0.
+// yields one of its own NaNs, and folding the representative in again in k_group_combine changes nothing.  The MIN / MAX
+// ops of the other widths start from it too (no sentinel per type).  Float SUM starts from +0.0 (dfd_b200.h): a group
+// of only -0.0 values sums to +0.0.
 __device__ __forceinline__ void state_init(const ReduceCol& c, char* dst, int64_t rep) {
     switch (c.op) {
         case DFD_AGG_SUM_I64: case DFD_AGG_SUM_F64: *(uint64_t*)dst = 0; break;
@@ -134,6 +137,16 @@ __device__ __forceinline__ void state_init(const ReduceCol& c, char* dst, int64_
         case DFD_AGG_MIN_I64: *(long long*)dst = 0x7fffffffffffffffLL; break;
         case DFD_AGG_MAX_I64: *(long long*)dst = (long long)0x8000000000000000ULL; break;
         case DFD_AGG_MIN_F64: case DFD_AGG_MAX_F64: *(uint64_t*)dst = *(const uint64_t*)(c.in + rep * 8); break;
+        default: {  // MIN / MAX of every other width (aligned to it, dfd_partial_reduce_device checks)
+            const char* src = c.in + rep * (int64_t)c.width;
+            switch (c.width) {
+                case 1: *dst = *src; break;
+                case 2: *(uint16_t*)dst = *(const uint16_t*)src; break;
+                case 4: *(uint32_t*)dst = *(const uint32_t*)src; break;
+                case 8: *(uint64_t*)dst = *(const uint64_t*)src; break;
+                default: ((uint64_t*)dst)[0] = ((const uint64_t*)src)[0]; ((uint64_t*)dst)[1] = ((const uint64_t*)src)[1]; break;
+            }
+        }
     }
 }
 
@@ -160,17 +173,83 @@ __global__ void __launch_bounds__(256) k_group_place(const __grid_constant__ Red
 // IEEE 754 totalOrder as a signed integer: flipping the magnitude bits of negative values makes the int64 order
 // -NaN < -inf < ... < -0.0 < +0.0 < ... < +inf < +NaN, with NaNs ordered by payload.  Only identical bits tie, so the
 // merged MIN / MAX is the same whatever order the rows arrive in.
-__device__ __forceinline__ long long f64_total_order_key(unsigned long long bits) {
-    return (long long)(bits ^ ((unsigned long long)((long long)bits >> 63) >> 1));
-}
-template <bool MAX>
-__device__ __forceinline__ void atomic_minmax_f64(unsigned long long* a, unsigned long long v) {
-    const long long vk = f64_total_order_key(v);
-    unsigned long long old = *a;
-    while (MAX ? vk > f64_total_order_key(old) : vk < f64_total_order_key(old)) {
-        const unsigned long long prev = atomicCAS(a, old, v);
+// Float32 / Float16 likewise at their width.
+struct TotalOrder {
+    __device__ long long operator()(unsigned long long bits) const {
+        return (long long)(bits ^ ((unsigned long long)((long long)bits >> 63) >> 1));
+    }
+    __device__ int operator()(unsigned bits) const { return (int)(bits ^ ((unsigned)((int)bits >> 31) >> 1)); }
+    __device__ short operator()(unsigned short bits) const { return (short)(bits ^ ((unsigned short)((short)bits >> 15) >> 1)); }
+};
+struct SignedOrder {
+    __device__ short operator()(unsigned short b) const { return (short)b; }
+    __device__ signed char operator()(unsigned char b) const { return (signed char)b; }
+};
+struct UnsignedOrder {
+    template <typename W> __device__ W operator()(W b) const { return b; }
+};
+
+// MIN / MAX of a 16-, 32- or 64-bit word by CAS, values compared as order(value).  The loop exits on a value a single load
+// or an atomic returned, and writes only when v wins, so the result is the bits of one input row.
+template <bool MAX, typename W, typename Order>
+__device__ __forceinline__ void atomic_minmax_cas(W* a, W v, Order order) {
+    const auto vk = order(v);
+    W old = *a;
+    while (MAX ? vk > order(old) : vk < order(old)) {
+        const W prev = atomicCAS(a, old, v);
         if (prev == old) break;
         old = prev;
+    }
+}
+
+// 1-byte MIN / MAX: CAS on the aligned 32-bit word that holds the byte, replacing that byte only.  The word's other bytes
+// may be other groups' rows, updated at the same moment (a CAS that loses to one of them retries with its new bytes), or
+// lie outside the column: a CAS stores them as it found them, and only if no byte of the word moved, so they never change.
+template <bool MAX, typename Order>
+__device__ __forceinline__ void atomic_minmax_u8(unsigned char* p, unsigned char v, Order order) {
+    unsigned* w = (unsigned*)((uintptr_t)p & ~(uintptr_t)3);
+    const unsigned sh = ((unsigned)(uintptr_t)p & 3u) * 8u;
+    const auto vk = order(v);
+    unsigned old = *w;
+    while (MAX ? vk > order((unsigned char)(old >> sh)) : vk < order((unsigned char)(old >> sh))) {
+        const unsigned prev = atomicCAS(w, old, (old & ~(0xffu << sh)) | ((unsigned)v << sh));
+        if (prev == old) break;
+        old = prev;
+    }
+}
+
+// One 128-bit compare-and-swap (sm_90, PTX ISA 8.3): *a = n if *a == c.  Returns the old value in (lo, hi).
+__device__ __forceinline__ void atomic_cas_b128(unsigned long long* a, unsigned long long& lo, unsigned long long& hi,
+                                                unsigned long long nlo, unsigned long long nhi) {
+    asm volatile(
+        "{\n\t.reg .b128 d, c, n;\n\t"
+        "mov.b128 c, {%0, %1};\n\t"
+        "mov.b128 n, {%3, %4};\n\t"
+        "atom.global.cas.b128 d, [%2], c, n;\n\t"
+        "mov.b128 {%0, %1}, d;\n\t}"
+        : "+l"(lo), "+l"(hi)
+        : "l"(__cvta_generic_to_global(a)), "l"(nlo), "l"(nhi)
+        : "memory");
+}
+
+// 128-bit MIN / MAX (Decimal128): CAS on the whole 16-byte word, never two 64-bit updates (unlike SUM_I128, a MIN / MAX
+// cannot be split into halves).  Order: the signed high halves, then the unsigned low halves.  Two 64-bit loads of the
+// word may tear, so the loop trusts them for one thing only: a state only moves towards its result, so a v that loses on
+// the high half alone, which one load reads whole, never wins.  Any other exit rests on a value the CAS returned: when v
+// does not beat the loaded guess, the CAS writes the guess back unchanged, which succeeds only if the guess was real.
+template <bool MAX>
+__device__ __forceinline__ void atomic_minmax_i128(unsigned long long* a, unsigned long long vlo, long long vhi) {
+    long long hi = *(volatile long long*)(a + 1);
+    if (MAX ? vhi < hi : vhi > hi) return;
+    unsigned long long lo = *(volatile unsigned long long*)a;
+    for (bool exact = false;; exact = true) {
+        const bool wins = MAX ? (vhi > hi || (vhi == hi && vlo > lo)) : (vhi < hi || (vhi == hi && vlo < lo));
+        if (!wins && exact) return;
+        unsigned long long plo = lo, phi = (unsigned long long)hi;
+        atomic_cas_b128(a, plo, phi, wins ? vlo : lo, wins ? (unsigned long long)vhi : (unsigned long long)hi);
+        if (plo == lo && (long long)phi == hi) return;
+        lo = plo;
+        hi = (long long)phi;
     }
 }
 
@@ -187,8 +266,32 @@ __global__ void __launch_bounds__(256) k_group_combine(const __grid_constant__ R
                 case DFD_AGG_SUM_F64: atomicAdd((double*)dst, *(const double*)src); break;
                 case DFD_AGG_MIN_I64: atomicMin((long long*)dst, *(const long long*)src); break;
                 case DFD_AGG_MAX_I64: atomicMax((long long*)dst, *(const long long*)src); break;
-                case DFD_AGG_MIN_F64: atomic_minmax_f64<false>((unsigned long long*)dst, *(const unsigned long long*)src); break;
-                case DFD_AGG_MAX_F64: atomic_minmax_f64<true>((unsigned long long*)dst, *(const unsigned long long*)src); break;
+                case DFD_AGG_MIN_F64: atomic_minmax_cas<false>((unsigned long long*)dst, *(const unsigned long long*)src, TotalOrder{}); break;
+                case DFD_AGG_MAX_F64: atomic_minmax_cas<true>((unsigned long long*)dst, *(const unsigned long long*)src, TotalOrder{}); break;
+                case DFD_AGG_MIN_I32: atomicMin((int*)dst, *(const int*)src); break;
+                case DFD_AGG_MAX_I32: atomicMax((int*)dst, *(const int*)src); break;
+                case DFD_AGG_MIN_U64: atomicMin((unsigned long long*)dst, *(const unsigned long long*)src); break;
+                case DFD_AGG_MAX_U64: atomicMax((unsigned long long*)dst, *(const unsigned long long*)src); break;
+                case DFD_AGG_MIN_U32: atomicMin((unsigned*)dst, *(const unsigned*)src); break;
+                case DFD_AGG_MAX_U32: atomicMax((unsigned*)dst, *(const unsigned*)src); break;
+                case DFD_AGG_MIN_I16: atomic_minmax_cas<false>((unsigned short*)dst, *(const unsigned short*)src, SignedOrder{}); break;
+                case DFD_AGG_MAX_I16: atomic_minmax_cas<true>((unsigned short*)dst, *(const unsigned short*)src, SignedOrder{}); break;
+                case DFD_AGG_MIN_U16: atomic_minmax_cas<false>((unsigned short*)dst, *(const unsigned short*)src, UnsignedOrder{}); break;
+                case DFD_AGG_MAX_U16: atomic_minmax_cas<true>((unsigned short*)dst, *(const unsigned short*)src, UnsignedOrder{}); break;
+                case DFD_AGG_MIN_F16: atomic_minmax_cas<false>((unsigned short*)dst, *(const unsigned short*)src, TotalOrder{}); break;
+                case DFD_AGG_MAX_F16: atomic_minmax_cas<true>((unsigned short*)dst, *(const unsigned short*)src, TotalOrder{}); break;
+                case DFD_AGG_MIN_I8: atomic_minmax_u8<false>((unsigned char*)dst, *(const unsigned char*)src, SignedOrder{}); break;
+                case DFD_AGG_MAX_I8: atomic_minmax_u8<true>((unsigned char*)dst, *(const unsigned char*)src, SignedOrder{}); break;
+                case DFD_AGG_MIN_U8: atomic_minmax_u8<false>((unsigned char*)dst, *(const unsigned char*)src, UnsignedOrder{}); break;
+                case DFD_AGG_MAX_U8: atomic_minmax_u8<true>((unsigned char*)dst, *(const unsigned char*)src, UnsignedOrder{}); break;
+                case DFD_AGG_MIN_F32: atomic_minmax_cas<false>((unsigned*)dst, *(const unsigned*)src, TotalOrder{}); break;
+                case DFD_AGG_MAX_F32: atomic_minmax_cas<true>((unsigned*)dst, *(const unsigned*)src, TotalOrder{}); break;
+                case DFD_AGG_MIN_I128:
+                    atomic_minmax_i128<false>((unsigned long long*)dst, ((const unsigned long long*)src)[0], ((const long long*)src)[1]);
+                    break;
+                case DFD_AGG_MAX_I128:
+                    atomic_minmax_i128<true>((unsigned long long*)dst, ((const unsigned long long*)src)[0], ((const long long*)src)[1]);
+                    break;
                 case DFD_AGG_SUM_I128: {
                     // two's complement 128-bit add as two 64-bit atomics: each add propagates its OWN carry exactly once
                     const unsigned long long lo = ((const unsigned long long*)src)[0], hi = ((const unsigned long long*)src)[1];
@@ -199,6 +302,21 @@ __global__ void __launch_bounds__(256) k_group_combine(const __grid_constant__ R
                 }
             }
         }
+    }
+}
+
+// Bytes of a state column of `op`; 0 for a value outside dfd_agg_op.
+int agg_width(int op) {
+    switch (op) {
+        case DFD_AGG_SUM_I128: case DFD_AGG_MIN_I128: case DFD_AGG_MAX_I128: return 16;
+        case DFD_AGG_SUM_I64: case DFD_AGG_SUM_F64: case DFD_AGG_MIN_I64: case DFD_AGG_MAX_I64: case DFD_AGG_MIN_F64:
+        case DFD_AGG_MAX_F64: case DFD_AGG_MIN_U64: case DFD_AGG_MAX_U64: return 8;
+        case DFD_AGG_MIN_I32: case DFD_AGG_MAX_I32: case DFD_AGG_MIN_U32: case DFD_AGG_MAX_U32: case DFD_AGG_MIN_F32:
+        case DFD_AGG_MAX_F32: return 4;
+        case DFD_AGG_MIN_I16: case DFD_AGG_MAX_I16: case DFD_AGG_MIN_U16: case DFD_AGG_MAX_U16: case DFD_AGG_MIN_F16:
+        case DFD_AGG_MAX_F16: return 2;
+        case DFD_AGG_MIN_I8: case DFD_AGG_MAX_I8: case DFD_AGG_MIN_U8: case DFD_AGG_MAX_U8: return 1;
+        default: return 0;
     }
 }
 
@@ -232,11 +350,18 @@ extern "C" int dfd_partial_reduce_device(dfd_ctx* c, const dfd_column* in_cols, 
         bool is_key = false;
         for (int k = 0; k < n_keys; ++k) is_key |= key_cols[k] == i;
         if (op < 0 && !is_key) return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d is neither a group key nor an aggregate state", i);
-        const int need = op < 0 ? ic.width : (op == DFD_AGG_SUM_I128 ? 16 : 8);
-        if (op > DFD_AGG_MAX_F64 || ic.width != need || (op < 0 && ic.width != 1 && ic.width != 2 && ic.width != 4 && ic.width != 8 && ic.width != 16))
+        const int need = op < 0 ? ic.width : agg_width(op);
+        if (op > DFD_AGG_MAX_F16 || ic.width != need || (op < 0 && ic.width != 1 && ic.width != 2 && ic.width != 4 && ic.width != 8 && ic.width != 16))
             return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: aggregate op %d does not match value width %d", i, op, ic.width);
         P.col[i] = ReduceCol{(const char*)ic.values + ic.offset * (int64_t)ic.width, (char*)out_cols[i].values, ic.width, op};
         if (!ic.values || !out_cols[i].values) return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: values is NULL", i);
+        // the MIN / MAX ops numbered 7 and up load and update whole values: each must sit at an address aligned
+        // to its width (an input 128-bit value, read as two 64-bit halves, to 8 bytes; an output one, a 128-bit atomic's
+        // target, to 16)
+        if (op >= DFD_AGG_MIN_I32 && ((uintptr_t)P.col[i].in % (uintptr_t)(ic.width < 8 ? ic.width : 8) != 0 ||
+                                      (uintptr_t)P.col[i].out % (uintptr_t)ic.width != 0))
+            return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: aggregate op %d needs values aligned to their width %d (input %p, output %p)",
+                             i, op, ic.width, (const void*)P.col[i].in, (void*)P.col[i].out);
     }
     std::lock_guard<std::mutex> lk(c->mu);
     cudaError_t e = cudaSetDevice(c->device);

@@ -144,6 +144,38 @@ class HashPartitioner:
         return np.frombuffer(starts, dtype=np.int64).copy(), np.frombuffer(counts, dtype=np.int64).copy()
 
 
+def agg_op(arrow_type, kind: str) -> int:
+    """The `nv.AGG_*` op that merges a partial aggregate state of Arrow type `arrow_type`, for `kind` "sum" (also COUNT
+    states, Int64) or "min" / "max" (a state of the aggregated column's type).  ValueError for a state with no device op:
+    strings, booleans, intervals, Decimal256, a SUM state DataFusion never makes, ..."""
+    import pyarrow as pa
+
+    t = pa.types
+    if kind == "sum":
+        if t.is_int64(arrow_type) or t.is_uint64(arrow_type):  # two's complement sums wrap alike
+            return nv.AGG_SUM_I64
+        if t.is_float64(arrow_type):
+            return nv.AGG_SUM_F64
+        if t.is_decimal128(arrow_type):
+            return nv.AGG_SUM_I128
+        raise ValueError(f"no device SUM for a state of type {arrow_type}")
+    if kind not in ("min", "max"):
+        raise ValueError(f"aggregate kind {kind!r}: expected 'sum', 'min' or 'max'")
+    ops = (  # (predicate, MIN op); every MAX op is its MIN op + 1
+        (lambda x: t.is_int64(x) or t.is_timestamp(x) or t.is_date64(x) or t.is_time64(x) or t.is_duration(x) or t.is_decimal64(x),
+         nv.AGG_MIN_I64),
+        (lambda x: t.is_int32(x) or t.is_date32(x) or t.is_time32(x) or t.is_decimal32(x), nv.AGG_MIN_I32),
+        (t.is_int16, nv.AGG_MIN_I16), (t.is_int8, nv.AGG_MIN_I8),
+        (t.is_uint64, nv.AGG_MIN_U64), (t.is_uint32, nv.AGG_MIN_U32), (t.is_uint16, nv.AGG_MIN_U16), (t.is_uint8, nv.AGG_MIN_U8),
+        (t.is_decimal128, nv.AGG_MIN_I128),
+        (t.is_float64, nv.AGG_MIN_F64), (t.is_float32, nv.AGG_MIN_F32), (t.is_float16, nv.AGG_MIN_F16),
+    )
+    for pred, op in ops:
+        if pred(arrow_type):
+            return op + (kind == "max")
+    raise ValueError(f"no device {kind.upper()} for a state of type {arrow_type}")
+
+
 class PartialReduceExec:
     """≙ AggregateExec(mode = PartialReduce) above the producers' hash RepartitionExec
     (src/distributed_planner/partial_reduce_below_network_shuffles.rs:17-100): merges rows with equal group keys inside

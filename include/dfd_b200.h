@@ -515,7 +515,22 @@ int dfd_exchange_phase_ms(dfd_exchange* x, double* out3, uint64_t* n_shuffles);
  * sum accumulator does the same has not been verified).  Float
  * MIN / MAX order values by IEEE 754 totalOrder (Rust's f64::total_cmp): -NaN < -inf < ... < -0.0 < +0.0 < ... < +inf
  * < +NaN, NaNs ordered by payload.  So a +NaN wins MAX and a -NaN wins MIN, -0.0 is below +0.0, an all-NaN group yields
- * one of its NaNs, and the result's bits are one input row's bits, the same on every run. */
+ * one of its NaNs, and the result's bits are one input row's bits, the same on every run.  The F32 / F16 ops follow the
+ * same rule at their width.
+ * A MIN / MAX state has the type of the aggregated column.  Arrow type of the state -> op (state column width):
+ *   COUNT; SUM of Int64 or UInt64 (both wrap mod 2^64 alike)          -> SUM_I64             (8 B)
+ *   SUM of Float64 / Decimal128                                        -> SUM_F64 / SUM_I128  (8 / 16 B)
+ *   Int64, Timestamp, Date64, Time64, Duration, Decimal64 MIN / MAX   -> MIN_I64 / MAX_I64   (8 B signed)
+ *   Int32, Date32, Time32, Decimal32 MIN / MAX                        -> MIN_I32 / MAX_I32   (4 B signed)
+ *   Int16 / Int8 MIN / MAX                                             -> MIN_I16 ... MAX_I8  (2 / 1 B signed)
+ *   UInt64 / UInt32 / UInt16 / UInt8 MIN / MAX                         -> MIN_U64 ... MAX_U8  (8 / 4 / 2 / 1 B unsigned)
+ *   Decimal128 MIN / MAX                                               -> MIN_I128 / MAX_I128 (16 B signed)
+ *   Float64 / Float32 / Float16 MIN / MAX                              -> MIN_F64 ... MAX_F16 (totalOrder)
+ * A state column must be exactly its op's width (else DFD_ERR_INVALID_ARGUMENT; so must an op outside the enum).  The
+ * MIN / MAX ops numbered 7 and up also need the address of every value aligned to its width (an input I128 value to 8
+ * bytes, an output one to 16: a 128-bit atomic's rule), else DFD_ERR_INVALID_ARGUMENT before anything is allocated or
+ * launched.  1-byte states have no alignment rule: they are updated through the aligned 32-bit word that holds them,
+ * and the other bytes of that word are never changed. */
 typedef enum {
     DFD_AGG_SUM_I64 = 0,  /* also COUNT states */
     DFD_AGG_SUM_F64 = 1,
@@ -523,7 +538,27 @@ typedef enum {
     DFD_AGG_MAX_I64 = 3,
     DFD_AGG_SUM_I128 = 4, /* Decimal128 sums */
     DFD_AGG_MIN_F64 = 5,
-    DFD_AGG_MAX_F64 = 6
+    DFD_AGG_MAX_F64 = 6,
+    DFD_AGG_MIN_I32 = 7,
+    DFD_AGG_MAX_I32 = 8,
+    DFD_AGG_MIN_I16 = 9,
+    DFD_AGG_MAX_I16 = 10,
+    DFD_AGG_MIN_I8 = 11,
+    DFD_AGG_MAX_I8 = 12,
+    DFD_AGG_MIN_U64 = 13,
+    DFD_AGG_MAX_U64 = 14,
+    DFD_AGG_MIN_U32 = 15,
+    DFD_AGG_MAX_U32 = 16,
+    DFD_AGG_MIN_U16 = 17,
+    DFD_AGG_MAX_U16 = 18,
+    DFD_AGG_MIN_U8 = 19,
+    DFD_AGG_MAX_U8 = 20,
+    DFD_AGG_MIN_I128 = 21, /* Decimal128 MIN / MAX */
+    DFD_AGG_MAX_I128 = 22,
+    DFD_AGG_MIN_F32 = 23,
+    DFD_AGG_MAX_F32 = 24,
+    DFD_AGG_MIN_F16 = 25,
+    DFD_AGG_MAX_F16 = 26
 } dfd_agg_op;
 int dfd_partial_reduce_device(dfd_ctx* ctx, const dfd_column* in_cols, int n_cols, int64_t n_rows, const int32_t* key_cols, int n_keys,
                               const int32_t* agg_ops, const int64_t* part_starts_device, uint32_t num_partitions,
