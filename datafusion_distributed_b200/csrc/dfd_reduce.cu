@@ -10,10 +10,15 @@
 //                    fixed-width keys — the keys themselves are never copied into the table)
 //   k_group_count    groups per destination partition (representatives only)      -> exclusive scan (host, N+1 values)
 //   k_group_place    every group gets an output row inside its partition; key columns copied, states initialised
-//   k_group_combine  every input row folds its states into its group's output row with atomics
+//   k_group_combine  every input row folds its states into its group's output row with atomics (k_combine_nullable, the
+//                    same code skipping null states and setting the output bits, when a state column has a bitmap)
 //                    (SUM i64 / f64 / i128 (two 64-bit adds with carry); MIN / MAX of signed and unsigned 8- to 64-bit
 //                    integers, of 128-bit decimals and of f16 / f32 / f64 under totalOrder: native atomicMin / atomicMax
 //                    at 32 and 64 bits, CAS loops at 8 (on the enclosing 32-bit word), 16 and 128 bits and for floats)
+//   k_group_clear    only when a MIN / MAX state column has an input bitmap: zeroes the value of every such state that
+//                    no valid row reached (it still holds the sentinel k_group_place started it from)
+// Nullable keys and states: a null key equals a null of its column and nothing else (its bytes are never read); a null
+// state is skipped, and an output state is valid when one of its group's input states is.
 // Integer / byte work; random access into an L2-resident table for the cardinalities PartialReduce is used for.
 #include <cuda_runtime.h>
 
@@ -34,8 +39,11 @@ constexpr uint32_t SLOT_EMPTY = 0xffffffffu;
 struct ReduceCol {
     const char* in;
     char* out;
+    const uint8_t* in_valid;  // input bitmap, or NULL; row r's bit is bit in_bit + r counted from this byte
+    uint32_t* out_valid;      // output bitmap (4-byte aligned), or NULL for a non-null output column
     int32_t width;
     int32_t op;  // dfd_agg_op, or -1 for a group key
+    int32_t in_bit;  // 0..7
 };
 
 struct ReduceParams {
@@ -44,6 +52,7 @@ struct ReduceParams {
     int32_t key_idx[MAX_KEYS];
     int32_t n_keys;
     int64_t n_rows;
+    int64_t n_groups;       // output rows (k_group_clear only)
     uint32_t N;
     uint32_t table_mask;
     uint32_t* table;        // [table_mask + 1] representative row of every slot
@@ -60,10 +69,25 @@ __device__ __forceinline__ uint64_t mix64(uint64_t x) {
     return x;
 }
 
+__device__ __forceinline__ bool valid_at(const ReduceCol& c, int64_t row) {
+    const int64_t b = (int64_t)c.in_bit + row;
+    return (c.in_valid[b >> 3] >> (b & 7)) & 1;
+}
+
+// Sets output row o's bit.  Other rows of the word belong to other groups, so the update is atomic.
+__device__ __forceinline__ void set_valid(uint32_t* bits, int64_t o) { atomicOr(bits + (o >> 5), 1u << (o & 31)); }
+
+constexpr uint64_t NULL_KEY_TAG = 0x6a09e667f3bcc909ULL;  // hashed in place of a null key's bytes
+
+template <bool NULLS>
 __device__ __forceinline__ uint64_t key_hash(const ReduceParams& P, int64_t row) {
     uint64_t h = 0x9e3779b97f4a7c15ULL;
     for (int k = 0; k < P.n_keys; ++k) {
         const ReduceCol& c = P.col[P.key_idx[k]];
+        if (NULLS && c.in_valid && !valid_at(c, row)) {
+            h = mix64(h ^ NULL_KEY_TAG);
+            continue;
+        }
         const char* p = c.in + row * (int64_t)c.width;
         switch (c.width) {
             case 8: h = mix64(h ^ *(const uint64_t*)p); break;
@@ -76,9 +100,15 @@ __device__ __forceinline__ uint64_t key_hash(const ReduceParams& P, int64_t row)
     return h;
 }
 
+template <bool NULLS>
 __device__ __forceinline__ bool keys_equal(const ReduceParams& P, int64_t a, int64_t b) {
     for (int k = 0; k < P.n_keys; ++k) {
         const ReduceCol& c = P.col[P.key_idx[k]];
+        if (NULLS && c.in_valid) {  // a null equals a null of the same column and nothing else
+            const bool va = valid_at(c, a);
+            if (va != valid_at(c, b)) return false;
+            if (!va) continue;
+        }
         const char* pa = c.in + a * (int64_t)c.width;
         const char* pb = c.in + b * (int64_t)c.width;
         bool eq;
@@ -103,21 +133,27 @@ __device__ __forceinline__ uint32_t partition_of(const int64_t* starts, uint32_t
     return lo;
 }
 
-__global__ void __launch_bounds__(256) k_group_insert(const __grid_constant__ ReduceParams P) {
+// Every kernel that reads or writes bitmaps has two launches of one body: NULLS = false is the code of a call without
+// them (k_group_insert / _place / _combine), NULLS = true the one of a call with them (k_*_nullable).
+template <bool NULLS>
+__device__ __forceinline__ void insert_rows(const ReduceParams& P) {
     for (int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; row < P.n_rows; row += (int64_t)gridDim.x * blockDim.x) {
-        uint32_t s = (uint32_t)key_hash(P, row) & P.table_mask;
+        uint32_t s = (uint32_t)key_hash<NULLS>(P, row) & P.table_mask;
         for (;;) {
             uint32_t rep = P.table[s];
             if (rep == SLOT_EMPTY) {
                 rep = atomicCAS(P.table + s, SLOT_EMPTY, (uint32_t)row);
                 if (rep == SLOT_EMPTY) break;  // this row represents a new group
             }
-            if (keys_equal(P, (int64_t)rep, row)) break;
+            if (keys_equal<NULLS>(P, (int64_t)rep, row)) break;
             s = (s + 1) & P.table_mask;
         }
         P.row_slot[row] = s;
     }
 }
+
+__global__ void __launch_bounds__(256) k_group_insert(const __grid_constant__ ReduceParams P) { insert_rows<false>(P); }
+__global__ void __launch_bounds__(256) k_insert_nullable(const __grid_constant__ ReduceParams P) { insert_rows<true>(P); }
 
 __global__ void __launch_bounds__(256) k_group_count(const __grid_constant__ ReduceParams P) {
     for (int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; s <= (int64_t)P.table_mask; s += (int64_t)gridDim.x * blockDim.x) {
@@ -126,18 +162,53 @@ __global__ void __launch_bounds__(256) k_group_count(const __grid_constant__ Red
     }
 }
 
+// The start of a MIN / MAX whose representative is null: the end of the op's order that every value can replace, so that
+// it stays only if no valid row reaches the state (k_group_clear then zeroes it) or if a valid row holds exactly these
+// bits.  Signed integers: the type's maximum / minimum; unsigned: all ones / 0; floats: totalOrder's top +NaN 0x7f..f /
+// bottom -NaN 0xf..f.  -> the low 64 bits; the I128 high halves (0x7f..f / 0x80..0) are set in state_init.  (MIN_I64 /
+// MAX_I64 always start from their sentinel, valid representative or not.)
+__device__ __forceinline__ uint64_t minmax_sentinel(int op) {
+    switch (op) {
+        case DFD_AGG_MIN_I32: return 0x7fffffffu;
+        case DFD_AGG_MAX_I32: return 0x80000000u;
+        case DFD_AGG_MIN_I16: return 0x7fffu;
+        case DFD_AGG_MAX_I16: return 0x8000u;
+        case DFD_AGG_MIN_I8: return 0x7fu;
+        case DFD_AGG_MAX_I8: return 0x80u;
+        case DFD_AGG_MIN_F64: return 0x7fffffffffffffffULL;
+        case DFD_AGG_MIN_F32: return 0x7fffffffu;
+        case DFD_AGG_MIN_F16: return 0x7fffu;
+        case DFD_AGG_MAX_F64: case DFD_AGG_MAX_F32: case DFD_AGG_MAX_F16: case DFD_AGG_MIN_U64: case DFD_AGG_MIN_U32:
+        case DFD_AGG_MIN_U16: case DFD_AGG_MIN_U8: case DFD_AGG_MIN_I128: return ~0ULL;  // (cut to the state's width)
+        default: return 0;  // MAX_U64 / U32 / U16 / U8, MAX_I128
+    }
+}
+
 // `rep` = the group's representative row.  Float MIN / MAX start from its value, not from +-inf: an all-NaN group then
 // yields one of its own NaNs, and folding the representative in again in k_group_combine changes nothing.  The MIN / MAX
-// ops of the other widths start from it too (no sentinel per type).  Float SUM starts from +0.0 (dfd_b200.h): a group
-// of only -0.0 values sums to +0.0.
-__device__ __forceinline__ void state_init(const ReduceCol& c, char* dst, int64_t rep) {
+// ops of the other widths start from it too (no sentinel per type), unless it is null.  Float SUM starts from +0.0
+// (dfd_b200.h): a group of only -0.0 values sums to +0.0.
+__device__ __forceinline__ void state_init(const ReduceCol& c, char* dst, int64_t rep, bool rep_valid) {
     switch (c.op) {
         case DFD_AGG_SUM_I64: case DFD_AGG_SUM_F64: *(uint64_t*)dst = 0; break;
         case DFD_AGG_SUM_I128: ((uint64_t*)dst)[0] = 0; ((uint64_t*)dst)[1] = 0; break;
         case DFD_AGG_MIN_I64: *(long long*)dst = 0x7fffffffffffffffLL; break;
         case DFD_AGG_MAX_I64: *(long long*)dst = (long long)0x8000000000000000ULL; break;
-        case DFD_AGG_MIN_F64: case DFD_AGG_MAX_F64: *(uint64_t*)dst = *(const uint64_t*)(c.in + rep * 8); break;
+        case DFD_AGG_MIN_F64: case DFD_AGG_MAX_F64:
+            if (rep_valid) { *(uint64_t*)dst = *(const uint64_t*)(c.in + rep * 8); break; }
+            [[fallthrough]];
         default: {  // MIN / MAX of every other width (aligned to it, dfd_partial_reduce_device checks)
+            if (!rep_valid) {
+                const uint64_t v = minmax_sentinel(c.op);
+                switch (c.width) {
+                    case 1: *(uint8_t*)dst = (uint8_t)v; break;
+                    case 2: *(uint16_t*)dst = (uint16_t)v; break;
+                    case 4: *(uint32_t*)dst = (uint32_t)v; break;
+                    case 8: *(uint64_t*)dst = v; break;
+                    default: ((uint64_t*)dst)[0] = v; ((uint64_t*)dst)[1] = c.op == DFD_AGG_MIN_I128 ? 0x7fffffffffffffffULL : 0x8000000000000000ULL; break;
+                }
+                break;
+            }
             const char* src = c.in + rep * (int64_t)c.width;
             switch (c.width) {
                 case 1: *dst = *src; break;
@@ -150,7 +221,8 @@ __device__ __forceinline__ void state_init(const ReduceCol& c, char* dst, int64_
     }
 }
 
-__global__ void __launch_bounds__(256) k_group_place(const __grid_constant__ ReduceParams P) {
+template <bool NULLS>
+__device__ __forceinline__ void place_groups(const ReduceParams& P) {
     for (int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; s <= (int64_t)P.table_mask; s += (int64_t)gridDim.x * blockDim.x) {
         const uint32_t rep = P.table[s];
         if (rep == SLOT_EMPTY) continue;
@@ -160,15 +232,20 @@ __global__ void __launch_bounds__(256) k_group_place(const __grid_constant__ Red
         for (int c = 0; c < P.n_cols; ++c) {
             const ReduceCol& col = P.col[c];
             char* dst = col.out + o * (int64_t)col.width;
-            if (col.op < 0) {
+            const bool valid = !NULLS || !col.in_valid || valid_at(col, (int64_t)rep);
+            if (col.op < 0) {  // a null key's row: bit clear, value bytes zero
                 const char* src = col.in + (int64_t)rep * col.width;
-                for (int b = 0; b < col.width; ++b) dst[b] = src[b];
+                for (int b = 0; b < col.width; ++b) dst[b] = valid ? src[b] : 0;
             } else {
-                state_init(col, dst, (int64_t)rep);
+                state_init(col, dst, (int64_t)rep, valid);
             }
+            if (NULLS && col.out_valid && valid) set_valid(col.out_valid, o);  // k_combine_nullable: the other valid rows
         }
     }
 }
+
+__global__ void __launch_bounds__(256) k_group_place(const __grid_constant__ ReduceParams P) { place_groups<false>(P); }
+__global__ void __launch_bounds__(256) k_place_nullable(const __grid_constant__ ReduceParams P) { place_groups<true>(P); }
 
 // IEEE 754 totalOrder as a signed integer: flipping the magnitude bits of negative values makes the int64 order
 // -NaN < -inf < ... < -0.0 < +0.0 < ... < +inf < +NaN, with NaNs ordered by payload.  Only identical bits tie, so the
@@ -253,12 +330,19 @@ __device__ __forceinline__ void atomic_minmax_i128(unsigned long long* a, unsign
     }
 }
 
-__global__ void __launch_bounds__(256) k_group_combine(const __grid_constant__ ReduceParams P) {
+template <bool NULLS>
+__device__ __forceinline__ void combine_rows(const ReduceParams& P) {
     for (int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; row < P.n_rows; row += (int64_t)gridDim.x * blockDim.x) {
         const int64_t o = (int64_t)P.slot_out[P.row_slot[row]];
         for (int c = 0; c < P.n_cols; ++c) {
             const ReduceCol& col = P.col[c];
             if (col.op < 0) continue;
+            if (NULLS && col.in_valid) {  // (then out_valid is set too: dfd_partial_reduce_device checks)
+                if (!valid_at(col, row)) continue;
+                // a plain load first, so that the rows of one hot group do not all queue on the bitmap word's atomic
+                uint32_t* w = col.out_valid + (o >> 5);
+                if (!((*w >> (o & 31)) & 1u)) atomicOr(w, 1u << (o & 31));
+            }
             const char* src = col.in + row * (int64_t)col.width;
             char* dst = col.out + o * (int64_t)col.width;
             switch (col.op) {
@@ -305,6 +389,33 @@ __global__ void __launch_bounds__(256) k_group_combine(const __grid_constant__ R
     }
 }
 
+__global__ void __launch_bounds__(256) k_group_combine(const __grid_constant__ ReduceParams P) { combine_rows<false>(P); }
+__global__ void __launch_bounds__(256) k_combine_nullable(const __grid_constant__ ReduceParams P) { combine_rows<true>(P); }
+
+__host__ __device__ __forceinline__ bool is_minmax(int op) {
+    return op >= 0 && op != DFD_AGG_SUM_I64 && op != DFD_AGG_SUM_F64 && op != DFD_AGG_SUM_I128;
+}
+
+// Zeroes the value of every MIN / MAX state (of a column with an input bitmap) that no valid row reached: it still holds
+// the sentinel k_group_place started it from.  Launched after k_group_combine, only when such a column exists.
+__global__ void __launch_bounds__(256) k_group_clear(const __grid_constant__ ReduceParams P) {
+    for (int64_t o = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; o < P.n_groups; o += (int64_t)gridDim.x * blockDim.x) {
+        for (int c = 0; c < P.n_cols; ++c) {
+            const ReduceCol& col = P.col[c];
+            if (!col.in_valid || !is_minmax(col.op)) continue;
+            if ((col.out_valid[o >> 5] >> (o & 31)) & 1u) continue;
+            char* dst = col.out + o * (int64_t)col.width;
+            switch (col.width) {
+                case 1: *(uint8_t*)dst = 0; break;
+                case 2: *(uint16_t*)dst = 0; break;
+                case 4: *(uint32_t*)dst = 0; break;
+                case 8: *(uint64_t*)dst = 0; break;
+                default: ((uint64_t*)dst)[0] = 0; ((uint64_t*)dst)[1] = 0; break;
+            }
+        }
+    }
+}
+
 // Bytes of a state column of `op`; 0 for a value outside dfd_agg_op.
 int agg_width(int op) {
     switch (op) {
@@ -342,10 +453,17 @@ extern "C" int dfd_partial_reduce_device(dfd_ctx* c, const dfd_column* in_cols, 
             return set_error(DFD_ERR_INVALID_ARGUMENT, "key column %d out of range or carries an aggregate", key_cols[k]);
         P.key_idx[k] = key_cols[k];
     }
+    // which kernels run their nullable code: a key column has an input bitmap (insert); any column has a bitmap (place); a
+    // state column has an input bitmap (combine); a MIN / MAX state column has one (k_group_clear runs)
+    bool null_keys = false, any_bitmap = false, null_states = false, clear = false;
     for (int i = 0; i < n_cols; ++i) {
         const dfd_column& ic = in_cols[i];
-        if (ic.kind != DFD_COL_FIXED || ic.validity || out_cols[i].kind != DFD_COL_FIXED || out_cols[i].width != ic.width)
-            return set_error(DFD_ERR_UNSUPPORTED, "column %d: partial reduce moves fixed-width non-null columns (keys and aggregate states)", i);
+        if (ic.kind != DFD_COL_FIXED || out_cols[i].kind != DFD_COL_FIXED || out_cols[i].width != ic.width)
+            return set_error(DFD_ERR_UNSUPPORTED, "column %d: partial reduce moves fixed-width columns (keys and aggregate states)", i);
+        if (ic.validity && !out_cols[i].validity)
+            return set_error(DFD_ERR_UNSUPPORTED, "column %d has a validity bitmap but its output has none (a non-null output column)", i);
+        if ((uintptr_t)out_cols[i].validity % 4 != 0)
+            return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: the output validity bitmap %p is not 4-byte aligned", i, (void*)out_cols[i].validity);
         const int op = agg_ops[i];
         bool is_key = false;
         for (int k = 0; k < n_keys; ++k) is_key |= key_cols[k] == i;
@@ -353,7 +471,13 @@ extern "C" int dfd_partial_reduce_device(dfd_ctx* c, const dfd_column* in_cols, 
         const int need = op < 0 ? ic.width : agg_width(op);
         if (op > DFD_AGG_MAX_F16 || ic.width != need || (op < 0 && ic.width != 1 && ic.width != 2 && ic.width != 4 && ic.width != 8 && ic.width != 16))
             return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: aggregate op %d does not match value width %d", i, op, ic.width);
-        P.col[i] = ReduceCol{(const char*)ic.values + ic.offset * (int64_t)ic.width, (char*)out_cols[i].values, ic.width, op};
+        P.col[i] = ReduceCol{(const char*)ic.values + ic.offset * (int64_t)ic.width, (char*)out_cols[i].values,
+                             ic.validity ? ic.validity + (ic.offset >> 3) : nullptr, (uint32_t*)out_cols[i].validity, ic.width, op,
+                             (int32_t)(ic.offset & 7)};
+        null_keys |= ic.validity && op < 0;
+        any_bitmap |= ic.validity || out_cols[i].validity;
+        null_states |= ic.validity && op >= 0;
+        clear |= ic.validity && is_minmax(op);
         if (!ic.values || !out_cols[i].values) return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: values is NULL", i);
         // the MIN / MAX ops numbered 7 and up load and update whole values: each must sit at an address aligned
         // to its width (an input 128-bit value, read as two 64-bit halves, to 8 bytes; an output one, a 128-bit atomic's
@@ -392,7 +516,10 @@ extern "C" int dfd_partial_reduce_device(dfd_ctx* c, const dfd_column* in_cols, 
     if ((e = cudaMemsetAsync(P.table, 0xff, slots * 4, s)) != cudaSuccess) return cuda_error(e, "cudaMemsetAsync(table)");
     if ((e = cudaMemsetAsync(P.group_count, 0, small_b, s)) != cudaSuccess) return cuda_error(e, "cudaMemsetAsync(counters)");
     const unsigned grid = (unsigned)(c->sm_count * 8);
-    k_group_insert<<<grid, 256, 0, s>>>(P);
+    if (null_keys)
+        k_insert_nullable<<<grid, 256, 0, s>>>(P);
+    else
+        k_group_insert<<<grid, 256, 0, s>>>(P);
     k_group_count<<<grid, 256, 0, s>>>(P);
     if ((e = cudaGetLastError()) != cudaSuccess) return cuda_error(e, "k_group_insert / k_group_count");
     std::vector<unsigned long long> counts(N);
@@ -406,10 +533,21 @@ extern "C" int dfd_partial_reduce_device(dfd_ctx* c, const dfd_column* in_cols, 
     if (out_part_starts_device &&
         (e = cudaMemcpyAsync(out_part_starts_device, out_part_starts_host, sizeof(int64_t) * (N + 1), cudaMemcpyHostToDevice, s)) != cudaSuccess)
         return cuda_error(e, "H2D out_starts");
-    k_group_place<<<grid, 256, 0, s>>>(P);
-    k_group_combine<<<grid, 256, 0, s>>>(P);
-    if ((e = cudaGetLastError()) != cudaSuccess) return cuda_error(e, "k_group_place / k_group_combine");
-    c->metrics.kernel_launches += 4;
+    P.n_groups = out_part_starts_host[N];
+    for (int i = 0; i < n_cols; ++i)  // the words of output rows [0, G); k_group_place and k_group_combine set the valid ones
+        if (P.col[i].out_valid && (e = cudaMemsetAsync(P.col[i].out_valid, 0, (size_t)((P.n_groups + 31) / 32) * 4, s)) != cudaSuccess)
+            return cuda_error(e, "cudaMemsetAsync(output validity)");
+    if (any_bitmap)
+        k_place_nullable<<<grid, 256, 0, s>>>(P);
+    else
+        k_group_place<<<grid, 256, 0, s>>>(P);
+    if (null_states)
+        k_combine_nullable<<<grid, 256, 0, s>>>(P);
+    else
+        k_group_combine<<<grid, 256, 0, s>>>(P);
+    if (clear) k_group_clear<<<grid, 256, 0, s>>>(P);
+    if ((e = cudaGetLastError()) != cudaSuccess) return cuda_error(e, "k_group_place / k_group_combine / k_group_clear");
+    c->metrics.kernel_launches += clear ? 5 : 4;
     if ((e = cudaStreamSynchronize(s)) != cudaSuccess) return cuda_error(e, "partial reduce");  // (out_part_starts_host is caller memory)
     return DFD_OK;
 }

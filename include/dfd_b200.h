@@ -507,7 +507,19 @@ int dfd_exchange_phase_ms(dfd_exchange* x, double* out3, uint64_t* n_shuffles);
  * per distinct key, partition p = rows [out_part_starts[p], out_part_starts[p+1]) of out_cols (capacity n_rows; row order
  * inside a partition is unspecified, like a hash aggregate's).  Feed it to dfd_exchange_gather(DFD_ROUTE_SHUFFLE) — the
  * rows never leave the GPU between Partial aggregation, repartition, PartialReduce and the exchange.
- * Fixed-width non-null keys and states (nullable group keys / states: DFD_ERR_UNSUPPORTED).  Synchronous.
+ * Fixed-width keys and states, each of them nullable.  Synchronous.
+ * Nulls: in_cols[c].validity (optional, no alignment rule) holds row r's bit at Arrow position offset + r, LSB first.
+ * out_cols[c].validity != NULL marks column c as nullable in the schema (as in dfd_exchange_gather); an input bitmap
+ * with a NULL output bitmap is DFD_ERR_UNSUPPORTED, an output bitmap not 4-byte aligned DFD_ERR_INVALID_ARGUMENT, both
+ * returned before anything is allocated or launched.  An output bitmap holds ceil(n_rows / 32) * 4 bytes; the call
+ * writes exactly the 32-bit words of output rows [0, G) (G = out_part_starts[N] groups), with the bits at and past G
+ * zero, and nothing when n_rows is 0.  Without an input bitmap all G bits are set.
+ *   Keys: a null equals a null of the same column and differs from every value, and the bytes under it are never read:
+ *   (NULL, 1), (1, NULL) and (NULL, NULL) are three groups.  A null key's output row has its bit clear and zero bytes.
+ *   States: a null state contributes nothing.  An output state is null iff every input state of its group is, and its
+ *   bytes are then zero; otherwise it is what the group's non-null states alone give under the rules below.
+ * Every output byte and bit of a group is the same on every run, but for the addition order of a float SUM.  Kernel
+ * launches: 4, and 5 when a MIN / MAX state column has an input bitmap (the fifth zeroes the states no valid row reached).
  * At most 2^31 rows per call (the group table has up to 2^32 slots of 32-bit indices); more: DFD_ERR_UNSUPPORTED,
  * returned before anything is allocated or launched.
  * Integer SUMs wrap (two's complement, mod 2^64 / 2^128).  Float SUM starts from +0.0 and adds the group's values in an
