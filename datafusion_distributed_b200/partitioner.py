@@ -42,9 +42,10 @@ class HashPartitioner:
         self.partitioning = partitioning
         self._h = C.c_void_p()
         keys = (C.c_int32 * len(partitioning.key_cols))(*partitioning.key_cols)
-        seeds_arr = (C.c_uint64 * 4)(*seeds) if seeds is not None else None
+        # ahash seeds (None: DataFusion's (0, 0, 0, 0)); dictionary values hash with them too (set_key_dictionary)
+        self._seeds = (C.c_uint64 * 4)(*seeds) if seeds is not None else None
         nv.check(nv.lib().dfd_partitioner_create(ctx.handle, partitioning.partition_count, keys,
-                                                 len(partitioning.key_cols), seeds_arr, C.byref(self._h)))
+                                                 len(partitioning.key_cols), self._seeds, C.byref(self._h)))
         ctx._adopt(self)
 
     def set_key_hash_mode(self, key_index: int, mode: int):
@@ -53,8 +54,8 @@ class HashPartitioner:
 
     def set_key_dictionary(self, key_index: int, dictionary_values, unsigned_index: bool = False):
         """Key column `key_index` holds dictionary INDICES of `dictionary_values` (a pyarrow Array, or None to make the key
-        plain again): hash the values once on the device (`dfd_hash_columns_device`) and let rows take
-        dict_hashes[index] (`dfd_partitioner_set_key_dictionary`) — DataFusion's hash_dictionary.  `unsigned_index`:
+        plain again): hash the values once on the device (`dfd_hash_columns_device`, with this partitioner's seeds) and let
+        rows take dict_hashes[index] (`dfd_partitioner_set_key_dictionary`) — DataFusion's hash_dictionary.  `unsigned_index`:
         the indices are UInt8/16/32/64 (read zero-extended) rather than Int8/16/32/64."""
         if not hasattr(self, "_dicts"):
             self._dicts = {}
@@ -70,7 +71,7 @@ class HashPartitioner:
         vals = DeviceColumn.from_arrow(self.ctx, dictionary_values)
         n = len(dictionary_values)
         hashes = self.ctx.alloc(max(n * 8, 8))
-        nv.check(nv.lib().dfd_hash_columns_device(self.ctx.handle, columns_to_c([vals]), 1, n, None, hashes.ptr))
+        nv.check(nv.lib().dfd_hash_columns_device(self.ctx.handle, columns_to_c([vals]), 1, n, self._seeds, hashes.ptr))
         nv.check(nv.lib().dfd_partitioner_set_key_dictionary(self._h, key_index, hashes.ptr, vals.validity or None, int(bool(unsigned_index))))
         self._dicts[key_index] = (vals, hashes)  # keep the device buffers alive
 

@@ -156,8 +156,8 @@ int dfd_partitioner_set_key_hash_mode(dfd_partitioner* p, int key_index, int mod
  * src/execution_plans/benchmarks/fixture.rs:13-33).  DataFusion's hash_dictionary hashes the dictionary VALUES once
  * (create_hashes over the values array) and every row takes dict_hashes[index]; a null index or a null dictionary value
  * leaves the running hash untouched.  Pass the INDICES as the (fixed-width, 1/2/4/8-byte) key column and declare its
- * dictionary here: dict_hashes_device = the values' hashes (dfd_hash_columns_device over the values column, asynchronous
- * on the context's stream), dict_validity_device = the values' validity bitmap or NULL, index_is_unsigned = nonzero for
+ * dictionary here: dict_hashes_device = the values' hashes (dfd_hash_columns_device over the values column with the seeds
+ * the partitioner was created with, asynchronous on the context's stream), dict_validity_device = the values' validity bitmap or NULL, index_is_unsigned = nonzero for
  * UInt8/16/32/64 indices (zero-extended; 0: Int8/16/32/64, sign-extended).  The pointers must stay valid while partition
  * calls use them; NULL hashes turn the key back into a plain one.  Interval(DayTime) / Interval(MonthDayNano) VALUES cannot
  * be hashed through dfd_hash_columns_device (see there).  As PAYLOAD the indices are a plain fixed-width column and the

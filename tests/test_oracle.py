@@ -8,7 +8,7 @@ import pytest
 
 from oracle import oracle as orc
 from oracle import oracle_py as op
-from tests.util import cfg2_columns, golden
+from tests.util import cfg2_columns, golden, seed_tuples
 
 
 def test_survey_8c_vectors():
@@ -62,6 +62,58 @@ def test_c_matches_python_restatement_randomised():
     sl = [c.slice(17, 300) for c in cols_c]
     slp = [(k, w, v[17:317]) for k, w, v in cols_p]
     assert orc.create_hashes(sl, 300).tolist() == op.create_hashes(slp, 300)
+
+
+@pytest.mark.parametrize("seeds", seed_tuples())
+def test_c_matches_python_restatement_seeded(seeds):
+    """The C oracle against the Python restatement under every seed tuple of the device hash tests: each column kind
+    alone (integers of 1 to 16 bytes, Boolean, Utf8, Binary, LargeUtf8, intervals), three keys in all 8 null patterns,
+    and the whole set sliced at Arrow offsets 1-7, 13 and 37."""
+    import struct
+
+    rnd = random.Random(sum(seeds) % 1009)
+    st = op.with_seeds(*seeds)
+    n = 240
+    nullable = lambda v, j: [None if (i >> j) % 2 and j < 3 else x for i, x in enumerate(v)]  # keys 0-2: r % 8's null pattern
+    ints = [(w, [rnd.getrandbits(8 * w) for _ in range(n)]) for w in (1, 2, 4, 8, 16)]
+    raw = [bytes(rnd.getrandbits(8) for _ in range(rnd.choice([0, 1, 3, 7, 8, 9, 16, 17, 33, 70]))) for _ in range(n)]
+    cols_p = [("str", 0, raw), ("bytes", 0, raw), ("bool", 1, [rnd.random() < 0.5 for _ in range(n)])]
+    cols_p += [("int", w, v) for w, v in ints]
+    cols_p += [("str", 0, [rnd.choice([None, b"", x]) for x in raw])]
+    cols_p = [(k, w, nullable(v, j)) for j, (k, w, v) in enumerate(cols_p)]
+
+    def to_arrow(kind, w, v, large=False):
+        if kind == "bool":
+            return pa.array(v, type=pa.bool_())
+        if kind == "int" and w == 16:
+            valid = np.array([x is not None for x in v])
+            data = b"".join((x or 0).to_bytes(16, "little") for x in v)
+            return pa.Array.from_buffers(pa.decimal128(38, 0), n, [pa.py_buffer(np.packbits(valid, bitorder="little").tobytes()),
+                                                                    pa.py_buffer(data)], null_count=int((~valid).sum()))
+        if kind == "int":
+            return pa.array(v, type={1: pa.uint8(), 2: pa.uint16(), 4: pa.uint32(), 8: pa.uint64()}[w])
+        b = pa.array(v, type=pa.binary())
+        if kind == "bytes":
+            return b
+        s = pa.Array.from_buffers(pa.string(), n, b.buffers(), null_count=b.null_count)
+        return s.cast(pa.large_string()) if large else s
+
+    cols_c = [to_arrow(*c) for c in cols_p]
+    large = to_arrow("str", 0, cols_p[0][2], large=True)
+    for c, p in [(large, cols_p[0])] + list(zip(cols_c, cols_p)):
+        assert orc.create_hashes([c], n, seeds).tolist() == op.create_hashes([p], n, st), (p[0], p[1])
+    assert orc.create_hashes(cols_c[:3], n, seeds).tolist() == op.create_hashes(cols_p[:3], n, st)
+    for off in [1, 2, 3, 4, 5, 6, 7, 13, 37]:
+        m = n - off - 3
+        sl = [c.slice(off, m) for c in cols_c]
+        slp = [(k, w, v[off:off + m]) for k, w, v in cols_p]
+        assert orc.create_hashes(sl, m, seeds).tolist() == op.create_hashes(slp, m, st), off
+    dt = [(rnd.getrandbits(32) - (1 << 31), rnd.getrandbits(32) - (1 << 31)) for _ in range(n)]
+    mdn = [(rnd.getrandbits(32) - (1 << 31), rnd.getrandbits(32) - (1 << 31), rnd.getrandbits(64) - (1 << 63)) for _ in range(n)]
+    h = orc.create_hashes([("interval_day_time", np.frombuffer(b"".join(struct.pack("<ii", *x) for x in dt), dtype=np.uint8))], n, seeds)
+    assert h.tolist() == [op.hash_one_interval_day_time(*x, st=st) for x in dt]
+    h = orc.create_hashes([("interval_month_day_nano", np.frombuffer(b"".join(struct.pack("<iiq", *x) for x in mdn), dtype=np.uint8))], n, seeds)
+    assert h.tolist() == [op.hash_one_interval_month_day_nano(*x, st=st) for x in mdn]
 
 
 def test_null_keys_keep_previous_hash():

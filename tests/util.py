@@ -19,6 +19,16 @@ def golden():
         return json.load(f)
 
 
+def seed_tuples():
+    """ahash seed tuples for the seeded hash tests: DataFusion's default (0, 0, 0, 0), the golden seeded states, each of
+    the four words set alone (a word swapped into another hasher field changes the hash), and four distinct words with
+    their high bits set."""
+    h = 0x9E3779B97F4A7C15
+    golden_seeds = sorted({tuple(e["seeds"]) for e in golden()["seeded"]})
+    return ([(0, 0, 0, 0)] + golden_seeds + [tuple(h if i == j else 0 for i in range(4)) for j in range(4)] +
+            [(0xF0E1D2C3B4A59687, 0x8899AABBCCDDEEFF, 0xC001D00DFEEDFACE, 0xDEADBEEF8BADF00D)])
+
+
 def cfg2_columns(n_rows: int, n_cols: int = 8, seed: int = 42):
     """SURVEY.md §8(d) cfg-2 shape: col0 = uniform i64 key, cols j>=1 = row_id*8+j."""
     rng = np.random.Generator(np.random.PCG64(seed))
