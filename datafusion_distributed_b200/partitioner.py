@@ -191,14 +191,15 @@ class PartialReduceExec:
         """-> (out_cols, out_part_starts[N+1]); `part_starts_device` = device pointer to the input's int64 part_starts[N+1].
         `nullable[i]` is the SCHEMA's nullable flag of column i (default: the columns of this batch that have a bitmap):
         the allocated output column i gets a validity bitmap when it is set, whether or not this batch has nulls, so that
-        the outputs of every batch have the same schema."""
+        the outputs of every batch have the same schema.  Group keys may be Boolean, Utf8, LargeUtf8 or Binary columns; an
+        allocated var-width key output holds as many bytes as its input."""
         if out_cols is None:
             out_cols = []
             for i, c in enumerate(cols):
                 o = DeviceColumn.empty_like(self.ctx, c, n_rows)
                 if (nullable[i] if nullable is not None else bool(c.validity)) and not o.validity:
                     vb = self.ctx.alloc(max((n_rows + 31) // 32 * 4, 4)).zero()  # (to_arrow reads the bitmap from keep[0])
-                    o = DeviceColumn(o.kind, o.width, o.values, 0, vb.ptr, 0, n_rows, [vb] + o.keep, o.arrow_type)
+                    o = DeviceColumn(o.kind, o.width, o.values, o.offsets, vb.ptr, 0, n_rows, [vb] + o.keep, o.arrow_type, o.values_bytes)
                 out_cols.append(o)
         keys = (C.c_int32 * len(self.key_cols))(*self.key_cols)
         ops = (C.c_int32 * len(self.agg_ops))(*self.agg_ops)

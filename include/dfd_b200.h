@@ -507,7 +507,21 @@ int dfd_exchange_phase_ms(dfd_exchange* x, double* out3, uint64_t* n_shuffles);
  * per distinct key, partition p = rows [out_part_starts[p], out_part_starts[p+1]) of out_cols (capacity n_rows; row order
  * inside a partition is unspecified, like a hash aggregate's).  Feed it to dfd_exchange_gather(DFD_ROUTE_SHUFFLE) — the
  * rows never leave the GPU between Partial aggregation, repartition, PartialReduce and the exchange.
- * Fixed-width keys and states, each of them nullable.  Synchronous.
+ * Keys: fixed-width (1/2/4/8/16 bytes), DFD_COL_BOOL, DFD_COL_UTF8, DFD_COL_LARGE_UTF8 or DFD_COL_BINARY; states:
+ * fixed-width; any of them nullable.  A Boolean or var-width state column is DFD_ERR_UNSUPPORTED.  Synchronous.
+ *   Var-width key: offsets plus bytes at any Arrow offset (the first offset may be nonzero, the bytes may start at any
+ *   address); keys are equal when their lengths and bytes are, so "", "a" and "a\0" are three groups and a null is not
+ *   "".  out_cols[c] has the input's kind; its `offsets` hold n_rows + 1 entries of the input's offset width, aligned to
+ *   it, of which the call writes exactly entries [0, G]; its `values` hold values_bytes bytes, of which exactly bytes
+ *   [0, total) are written: group o's bytes are its representative row's, a null key's row is empty.  If the groups'
+ *   total key bytes exceed values_bytes, the call returns DFD_ERR_CAPACITY (the message names the bytes needed) before
+ *   any output is written, out_part_starts included; the input's own byte count is always enough.
+ *   Boolean key: bit-packed values at any bit offset.  The output follows dfd_partition_device's bit-packed outputs: 4-byte
+ *   aligned, ceil(n_rows / 32) * 4 bytes, of which exactly the words of rows [0, G) are written, the bits at and past G
+ *   zero.
+ *   An output kind that differs from its input's, NULL offsets, or a Boolean output not 4-byte aligned is
+ *   DFD_ERR_INVALID_ARGUMENT, returned before anything is allocated or launched.  With n_rows = 0, entry 0 of every
+ *   var-width key's offsets is set to 0.
  * Nulls: in_cols[c].validity (optional, no alignment rule) holds row r's bit at Arrow position offset + r, LSB first.
  * out_cols[c].validity != NULL marks column c as nullable in the schema (as in dfd_exchange_gather); an input bitmap
  * with a NULL output bitmap is DFD_ERR_UNSUPPORTED, an output bitmap not 4-byte aligned DFD_ERR_INVALID_ARGUMENT, both
@@ -519,7 +533,9 @@ int dfd_exchange_phase_ms(dfd_exchange* x, double* out3, uint64_t* n_shuffles);
  *   States: a null state contributes nothing.  An output state is null iff every input state of its group is, and its
  *   bytes are then zero; otherwise it is what the group's non-null states alone give under the rules below.
  * Every output byte and bit of a group is the same on every run, but for the addition order of a float SUM.  Kernel
- * launches: 4, and 5 when a MIN / MAX state column has an input bitmap (the fifth zeroes the states no valid row reached).
+ * launches: 4, and 5 when a MIN / MAX state column has an input bitmap (the fifth zeroes the states no valid row reached),
+ * + 4 per var-width key (an offset scan of 3 and a byte copy, one column at a time); a Boolean key adds none.  A call
+ * refused with DFD_ERR_CAPACITY has made 2 (the insert and the count).  None when n_rows is 0.
  * At most 2^31 rows per call (the group table has up to 2^32 slots of 32-bit indices); more: DFD_ERR_UNSUPPORTED,
  * returned before anything is allocated or launched.
  * Integer SUMs wrap (two's complement, mod 2^64 / 2^128).  Float SUM starts from +0.0 and adds the group's values in an
