@@ -27,6 +27,7 @@
 #include <dlfcn.h>
 #include <nccl.h>
 
+#include <algorithm>
 #include <cstring>
 #include <mutex>
 #include <new>
@@ -306,6 +307,50 @@ __global__ void __launch_bounds__(PUSH_THREADS) k_push_runs(const PushRun* __res
     }
 }
 
+// One bitmap run of dfd_shuffle_host's compaction: bits [0, n) of the word-aligned `src` land on bits [dst_bit, dst_bit + n)
+// of `dst`, at any destination bit.  A destination word the run covers whole is stored; the first and last words, which
+// the run shares with its neighbours, are OR-ed in with atomicOr (the caller zeroes the destination first).
+struct BitRun {
+    const unsigned* src;
+    unsigned* dst;
+    long long dst_bit, n;
+    int first_block;  // first CTA of this run in the launch (prefix over the runs)
+};
+constexpr long long BIT_WORDS_PER_CTA = 4 * PUSH_THREADS;
+
+__host__ __device__ inline long long bit_run_words(const BitRun& r) { return ((r.dst_bit & 31) + r.n + 31) >> 5; }
+
+__global__ void __launch_bounds__(PUSH_THREADS) k_place_bits(const BitRun* __restrict__ runs, int n_runs) {
+    int lo = 0, hi = n_runs;
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (runs[mid].first_block <= (int)blockIdx.x) lo = mid; else hi = mid;
+    }
+    const BitRun r = runs[lo];
+    const unsigned sh = (unsigned)(r.dst_bit & 31);
+    const long long n_src = (r.n + 31) >> 5;
+    const long long w0 = (long long)((int)blockIdx.x - r.first_block) * BIT_WORDS_PER_CTA;
+    const long long w_end = bit_run_words(r);
+    const long long w1 = w0 + BIT_WORDS_PER_CTA < w_end ? w0 + BIT_WORDS_PER_CTA : w_end;
+    unsigned* dw = r.dst + (r.dst_bit >> 5);
+    for (long long t = w0 + threadIdx.x; t < w1; t += PUSH_THREADS) {
+        // destination word t holds run bits [32 t - sh, 32 t - sh + 32)
+        const unsigned cur = t < n_src ? r.src[t] : 0u;
+        const unsigned prev = sh != 0 && t > 0 ? r.src[t - 1] : 0u;
+        const unsigned v = sh ? __funnelshift_l(prev, cur, sh) : cur;
+        const long long b0 = 32 * t - (long long)sh;  // run bit at bit 0 of this word
+        const unsigned first = t == 0 ? sh : 0u;
+        const long long left = r.n - b0;
+        const unsigned last = left < 32 ? (unsigned)left : 32u;  // one past the last bit of the run in this word
+        if (first == 0 && last == 32) {
+            dw[t] = v;
+        } else {
+            const unsigned mask = (last == 32 ? 0xffffffffu : (1u << last) - 1u) & ~((1u << first) - 1u);
+            atomicOr(dw + t, v & mask);
+        }
+    }
+}
+
 }  // namespace
 
 struct dfd_exchange {
@@ -366,6 +411,12 @@ struct dfd_exchange {
     cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
     cudaEvent_t e_h2d[2] = {}, e_k[2] = {}, e_d2h[2] = {};
     Scratch in_stage[2];
+    // dfd_shuffle_host over the push transport: the dense chunks compacted from the window, and their run lists
+    cudaEvent_t e_out[2] = {};
+    Scratch out_stage[2];
+    void* d_cruns = nullptr;
+    void* h_cruns = nullptr;  // pinned
+    size_t cruns_cap = 0;
     uint64_t bytes_sent = 0, bytes_received = 0, shuffles = 0;
 };
 
@@ -487,10 +538,15 @@ void dfd_exchange_destroy(dfd_exchange* x) {
         cudaFree(x->bytes_all.ptr);
         cudaFree(x->in_stage[0].ptr);
         cudaFree(x->in_stage[1].ptr);
+        cudaFree(x->out_stage[0].ptr);
+        cudaFree(x->out_stage[1].ptr);
+        cudaFree(x->d_cruns);
+        cudaFreeHost(x->h_cruns);
         for (int i = 0; i < 2; ++i) {
             if (x->e_h2d[i]) cudaEventDestroy(x->e_h2d[i]);
             if (x->e_k[i]) cudaEventDestroy(x->e_k[i]);
             if (x->e_d2h[i]) cudaEventDestroy(x->e_d2h[i]);
+            if (x->e_out[i]) cudaEventDestroy(x->e_out[i]);
         }
         if (x->s_h2d) cudaStreamDestroy(x->s_h2d);
         if (x->s_d2h) cudaStreamDestroy(x->s_d2h);
@@ -1314,11 +1370,356 @@ int dfd_shuffle_device(dfd_exchange* x, dfd_partitioner* part, int mode, const d
     return DFD_OK;
 }
 
+// ---- dfd_shuffle_host for nullable, Boolean and string columns: the push transport, chunk by chunk ----------------------
+// Per chunk i (rows [lo, hi) of every producer):
+//   1. H2D into input stage i & 1, every column at row offset lo & 7, so that bitmaps travel as the whole bytes that
+//      cover bits [lo, hi); string columns bring offsets [lo, hi] as they are and bytes [off[lo], off[hi]), their values
+//      pointer set back by off[lo] (the host reads both ends from its own memory: no read-back);
+//   2. push_shuffle_locked: local partition, then every destination's runs into its owner's window (whole window);
+//   3. compaction of this worker's P x T window segments into one dense chunk in an output stage: values, string bytes and
+//      re-based offsets through k_push_runs, bitmaps through k_place_bits at the chunk's host bit (out_row & 31, plus the
+//      previous chunk's bits of the host word the two chunks share, taken from the other output stage); then D2H.
+// H2D of chunk i+1 overlaps the shuffle of chunk i; D2H of chunk i overlaps the shuffle of chunk i+1.
+namespace {
+
+// A schema with any nullable, Boolean or string column takes the push transport (every worker decides the same way: the
+// nullable flags are the schema's, out_cols[c].validity on entry).
+bool host_shuffle_needs_push(const dfd_column* in_cols, const dfd_column* out_cols, int n_cols) {
+    for (int i = 0; i < n_cols; ++i)
+        if (in_cols[i].kind != DFD_COL_FIXED || in_cols[i].validity || out_cols[i].validity) return true;
+    return false;
+}
+
+bool is_var_kind(int kind) { return kind == DFD_COL_UTF8 || kind == DFD_COL_LARGE_UTF8 || kind == DFD_COL_BINARY; }
+
+int64_t host_offset(const dfd_column& c, int64_t row) {
+    return c.kind == DFD_COL_LARGE_UTF8 ? ((const int64_t*)c.offsets)[row] : (int64_t)((const int32_t*)c.offsets)[row];
+}
+
+int check_host_push_columns(const dfd_column* in_cols, const dfd_column* out_cols, int n_cols, int64_t n_rows) {
+    for (int i = 0; i < n_cols; ++i) {
+        const dfd_column& ic = in_cols[i];
+        const dfd_column& oc = out_cols[i];
+        if (ic.offset != 0) return set_error(DFD_ERR_UNSUPPORTED, "column %d: dfd_shuffle_host takes columns at Arrow offset 0", i);
+        if (ic.kind == DFD_COL_FIXED) {
+            if (ic.width != 1 && ic.width != 2 && ic.width != 4 && ic.width != 8 && ic.width != 16)
+                return set_error(DFD_ERR_UNSUPPORTED, "column %d: fixed width %d not in {1,2,4,8,16}", i, ic.width);
+        } else if (ic.kind != DFD_COL_BOOL && !is_var_kind(ic.kind)) {
+            return set_error(DFD_ERR_UNSUPPORTED, "column %d: unknown column kind %d", i, ic.kind);
+        }
+        if (oc.kind != ic.kind || (ic.kind == DFD_COL_FIXED && oc.width != ic.width))
+            return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: out layout mismatch", i);
+        if (ic.validity && !oc.validity)
+            return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: input has a validity bitmap but out validity is NULL (nullable columns need "
+                                                       "a validity buffer on EVERY worker)", i);
+        if (is_var_kind(ic.kind)) {
+            if (!ic.offsets || !oc.offsets) return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: offsets is NULL", i);
+            if ((host_offset(ic, n_rows) - host_offset(ic, 0) > 0 && !ic.values) || (oc.values_bytes > 0 && !oc.values))
+                return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: values is NULL", i);
+        } else if ((n_rows > 0 && !ic.values) || !oc.values) {
+            return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: values is NULL", i);
+        }
+    }
+    return DFD_OK;
+}
+
+}  // namespace
+
+static int host_push_chunks_locked(dfd_exchange* x, dfd_partitioner* part, const dfd_column* in_cols, int n_cols, int64_t n_rows,
+                                   uint32_t P, int n_chunks, const dfd_column* out_cols, int64_t out_capacity_rows,
+                                   int64_t* chunk_part_starts) {
+    dfd_ctx* c = x->ctx;
+    cudaStream_t s = c->stream;
+    const int T = x->world;
+    const uint32_t NS = P * (uint32_t)T;
+    if (!x->window_ready) return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_shuffle_host needs dfd_exchange_setup_window first");
+    auto chunk_lo = [&](int i) { return (int64_t)((__int128)n_rows * i / n_chunks); };
+    // ---- both input stages, sized once from the largest chunk
+    int64_t max_rows = 0;
+    std::vector<int64_t> max_bytes(n_cols, 0);
+    for (int i = 0; i < n_chunks; ++i) {
+        const int64_t lo = chunk_lo(i), hi = chunk_lo(i + 1);
+        max_rows = std::max(max_rows, hi - lo);
+        for (int k = 0; k < n_cols; ++k) {
+            if (!is_var_kind(in_cols[k].kind)) continue;
+            const int64_t nb = host_offset(in_cols[k], hi) - host_offset(in_cols[k], lo);
+            if (nb < 0) return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: offsets are not monotonic", k);
+            max_bytes[k] = std::max(max_bytes[k], nb);
+        }
+    }
+    std::vector<size_t> st_values(n_cols), st_off(n_cols), st_valid(n_cols);
+    size_t stage_bytes = 0;
+    const size_t bm = al((size_t)(max_rows + 7) / 8 + 1 + 16);  // the bytes covering bits [lo, hi), read as whole words
+    for (int k = 0; k < n_cols; ++k) {
+        const dfd_column& ic = in_cols[k];
+        const size_t ow = ic.kind == DFD_COL_LARGE_UTF8 ? 8 : 4;
+        if (ic.kind == DFD_COL_FIXED) { st_values[k] = stage_bytes; stage_bytes += al((size_t)(max_rows + 8) * ic.width + 16); }
+        else if (ic.kind == DFD_COL_BOOL) { st_values[k] = stage_bytes; stage_bytes += bm; }
+        else {
+            st_off[k] = stage_bytes; stage_bytes += al((size_t)(max_rows + 9) * ow + 16);
+            st_values[k] = stage_bytes; stage_bytes += al((size_t)max_bytes[k] + 32);
+        }
+        if (ic.validity) { st_valid[k] = stage_bytes; stage_bytes += bm; }
+    }
+    int rc;
+    for (int k = 0; k < 2; ++k)
+        if ((rc = x->in_stage[k].ensure(stage_bytes + 256, c->device))) return rc;
+    std::vector<dfd_column> dev_in[2] = {std::vector<dfd_column>(n_cols), std::vector<dfd_column>(n_cols)};
+    auto issue_h2d = [&](int i) -> int {
+        const int k = i & 1;
+        const int64_t lo = chunk_lo(i), hi = chunk_lo(i + 1), rows = hi - lo, sh = lo & 7;
+        const size_t b0 = (size_t)(lo >> 3), nb8 = (size_t)((hi + 7) >> 3) - b0;
+        if (i >= 2) CUDA_TRY(cudaStreamWaitEvent(x->s_h2d, x->e_k[k], 0), "wait");  // the partition of chunk i-2 read this stage
+        char* base = (char*)x->in_stage[k].ptr;
+        for (int cidx = 0; cidx < n_cols; ++cidx) {
+            const dfd_column& ic = in_cols[cidx];
+            dfd_column& d = dev_in[k][cidx];
+            d = ic;
+            d.offset = sh;
+            d.values = base + st_values[cidx];
+            if (ic.kind == DFD_COL_FIXED) {
+                const size_t w = (size_t)ic.width;
+                if (rows)
+                    CUDA_TRY(cudaMemcpyAsync(base + st_values[cidx] + (size_t)sh * w, (const char*)ic.values + (size_t)lo * w, (size_t)rows * w,
+                                             cudaMemcpyHostToDevice, x->s_h2d), "H2D");
+            } else if (ic.kind == DFD_COL_BOOL) {
+                if (rows) CUDA_TRY(cudaMemcpyAsync(base + st_values[cidx], (const char*)ic.values + b0, nb8, cudaMemcpyHostToDevice, x->s_h2d), "H2D");
+            } else {
+                const size_t ow = ic.kind == DFD_COL_LARGE_UTF8 ? 8 : 4;
+                const int64_t first = host_offset(ic, lo), nbytes = host_offset(ic, hi) - first;
+                d.offsets = base + st_off[cidx];
+                CUDA_TRY(cudaMemcpyAsync(base + st_off[cidx] + (size_t)sh * ow, (const char*)ic.offsets + (size_t)lo * ow, (size_t)(rows + 1) * ow,
+                                         cudaMemcpyHostToDevice, x->s_h2d), "H2D");
+                // bytes [first, first + nbytes) at the same address mod 16 as on the host; the offsets index them unchanged
+                char* bytes = base + st_values[cidx] + (first & 15);
+                if (nbytes) CUDA_TRY(cudaMemcpyAsync(bytes, (const char*)ic.values + first, (size_t)nbytes, cudaMemcpyHostToDevice, x->s_h2d), "H2D");
+                d.values = (void*)((uintptr_t)bytes - (uintptr_t)first);
+                d.values_bytes = nbytes;
+            }
+            if (ic.validity) {
+                d.validity = (uint8_t*)(base + st_valid[cidx]);
+                if (rows) CUDA_TRY(cudaMemcpyAsync(d.validity, ic.validity + b0, nb8, cudaMemcpyHostToDevice, x->s_h2d), "H2D");
+            }
+        }
+        CUDA_TRY(cudaEventRecord(x->e_h2d[k], x->s_h2d), "record");
+        return DFD_OK;
+    };
+    // ---- the output: entry 0 of a string column's offsets is 0 (written with the first rows, or once every chunk is through);
+    // entry out_row + k + 1 comes from the chunk that delivers host row out_row + k
+    std::vector<int> var_index(n_cols, -1);
+    int V = 0;
+    for (int k = 0; k < n_cols; ++k)
+        if (is_var_kind(in_cols[k].kind)) var_index[k] = V++;
+    auto first_offsets = [&] {
+        for (int k = 0; k < n_cols; ++k) {
+            if (in_cols[k].kind == DFD_COL_LARGE_UTF8) *(int64_t*)out_cols[k].offsets = 0;
+            else if (var_index[k] >= 0) *(int32_t*)out_cols[k].offsets = 0;
+        }
+    };
+    int64_t out_row = 0;
+    std::vector<int64_t> out_bytes(V, 0);
+    int last = -1;                 // output stage holding the last chunk that delivered rows
+    int64_t last_word = 0;         // its word 0 = host bitmap word last_word
+    bool stage_used[2] = {false, false};
+    std::vector<size_t> lane_off[2];  // per output stage: byte offset of every bitmap lane
+    if ((rc = issue_h2d(0))) return rc;
+    for (int i = 0; i < n_chunks; ++i) {
+        const int k = i & 1;
+        if (i + 1 < n_chunks && (rc = issue_h2d(i + 1))) return rc;
+        const int64_t rows = chunk_lo(i + 1) - chunk_lo(i);
+        CUDA_TRY(cudaStreamWaitEvent(s, x->e_h2d[k], 0), "wait");
+        std::vector<dfd_column> win(n_cols);
+        for (int cidx = 0; cidx < n_cols; ++cidx)
+            win[cidx].validity = in_cols[cidx].validity || out_cols[cidx].validity ? (uint8_t*)1 : nullptr;  // the schema's flag
+        if ((rc = push_shuffle_locked(x, part, dev_in[k].data(), n_cols, rows, P, win.data()))) return rc;
+        CUDA_TRY(cudaEventRecord(x->e_k[k], s), "record");
+        // this worker's segments q * T + r (producers in task order within each partition) and their bytes, in the window's
+        // layout (push_slices_locked: a column's byte segments back to back, each start rounded up to 16 bytes)
+        const std::vector<int64_t> seg_start = x->pending.seg_starts, seg_count = x->pending.seg_counts;
+        x->pending.kind = dfd_exchange::Pending::NONE;
+        std::vector<int64_t> bseg((size_t)V * NS, 0), bcnt((size_t)V * NS, 0), chunk_bytes(V, 0);
+        for (int v = 0; v < V; ++v) {
+            int64_t brun = 0;
+            for (uint32_t sg = 0; sg < NS; ++sg) {
+                const int r = (int)(sg % (uint32_t)T);
+                const uint32_t g = (uint32_t)x->rank * P + sg / (uint32_t)T;
+                const int64_t nb = x->h_meta[(size_t)r * XCHG_META_MAX + (size_t)NS * (1 + v) + g];
+                bseg[(size_t)v * NS + sg] = brun;
+                bcnt[(size_t)v * NS + sg] = nb;
+                brun = (brun + nb + 15) / 16 * 16;
+                chunk_bytes[v] += nb;
+            }
+        }
+        int64_t got = 0;
+        for (uint32_t sg = 0; sg < NS; ++sg) got += seg_count[sg];
+        // ---- this worker's host capacity (its peers learn of a refusal through their bounded flag waits)
+        if (out_row + got > out_capacity_rows)
+            return set_error(DFD_ERR_CAPACITY, "dfd_shuffle_host: out buffers hold %lld rows, need %lld", (long long)out_capacity_rows,
+                             (long long)(out_row + got));
+        for (int cidx = 0; cidx < n_cols; ++cidx) {
+            const int v = var_index[cidx];
+            if (v < 0) continue;
+            const int64_t need = out_bytes[v] + chunk_bytes[v];
+            if (need > out_cols[cidx].values_bytes)
+                return set_error(DFD_ERR_CAPACITY, "dfd_shuffle_host: column %d: out values_bytes is %lld, need %lld string bytes", cidx,
+                                 (long long)out_cols[cidx].values_bytes, (long long)need);
+            if (in_cols[cidx].kind != DFD_COL_LARGE_UTF8 && need > INT32_MAX)
+                return set_error(DFD_ERR_CAPACITY, "dfd_shuffle_host: column %d: string offsets would reach %lld, past the int32 offsets of "
+                                                   "Utf8 / Binary", cidx, (long long)need);
+        }
+        int64_t a = out_row;
+        for (uint32_t q = 0; q <= P; ++q) {
+            chunk_part_starts[(size_t)i * (P + 1) + q] = a;
+            for (int r = 0; q < P && r < T; ++r) a += seg_count[(size_t)q * T + r];
+        }
+        if (got > 0) {
+            if (out_row == 0) first_offsets();
+            // ---- compaction into output stage `cur` (not the one the previous chunk's bits are folded from)
+            const int cur = last < 0 ? 0 : last ^ 1;
+            if (stage_used[cur]) CUDA_TRY(cudaStreamWaitEvent(s, x->e_d2h[cur], 0), "wait");  // its D2H has drained it
+            if ((rc = x->out_stage[cur].ensure(x->window_bytes + 256, c->device))) return rc;
+            char* ob = (char*)x->out_stage[cur].ptr;
+            const unsigned sh0 = (unsigned)(out_row & 31);
+            const int64_t nw = (sh0 + got + 31) / 32;  // host bitmap words [out_row >> 5, + nw)
+            // layout: every bitmap lane first (one memset zeroes them), then values, offsets and string bytes.  Each region is
+            // no larger than the column's region in the window, so the stage holds window_bytes.
+            std::vector<size_t> o_val(n_cols), o_off(n_cols), o_bits(n_cols), o_valid(n_cols);
+            std::vector<size_t>& lanes = lane_off[cur];
+            lanes.clear();
+            size_t off = 0;
+            for (int cidx = 0; cidx < n_cols; ++cidx) {
+                if (in_cols[cidx].kind == DFD_COL_BOOL) { o_bits[cidx] = off; lanes.push_back(off); off += al((size_t)nw * 4); }
+                if (win[cidx].validity) { o_valid[cidx] = off; lanes.push_back(off); off += al((size_t)nw * 4); }
+            }
+            const size_t bits_bytes = off;
+            for (int cidx = 0; cidx < n_cols; ++cidx) {
+                const dfd_column& ic = in_cols[cidx];
+                const int v = var_index[cidx];
+                if (ic.kind == DFD_COL_FIXED) { o_val[cidx] = off; off += al((size_t)got * ic.width); }
+                else if (v >= 0) {
+                    o_off[cidx] = off; off += al((size_t)got * (ic.kind == DFD_COL_LARGE_UTF8 ? 8 : 4));
+                    o_val[cidx] = off; off += al((size_t)chunk_bytes[v]);
+                }
+            }
+            if (off > x->out_stage[cur].bytes) return set_error(DFD_ERR_INTERNAL, "dfd_shuffle_host: output stage of %zu B < %zu B", x->out_stage[cur].bytes, off);
+            if (bits_bytes) CUDA_TRY(cudaMemsetAsync(ob, 0, bits_bytes, s), "memset output bitmaps");
+            std::vector<PushRun> runs;
+            std::vector<BitRun> bruns;
+            auto bit_run = [&](const char* src_bitmap, int64_t seg, size_t dst_off, int64_t dst_bit, int64_t n) {
+                BitRun b{};
+                b.src = (const unsigned*)src_bitmap + seg / 32;  // segments start on 32-row boundaries
+                b.dst = (unsigned*)(ob + dst_off);
+                b.dst_bit = dst_bit;
+                b.n = n;
+                bruns.push_back(b);
+            };
+            int64_t drow = 0;
+            std::vector<int64_t> dbytes(V, 0);
+            for (uint32_t sg = 0; sg < NS; ++sg) {
+                const int64_t cnt = seg_count[sg], seg = seg_start[sg];
+                if (cnt == 0) continue;
+                for (int cidx = 0; cidx < n_cols; ++cidx) {
+                    const dfd_column& ic = in_cols[cidx];
+                    const dfd_column& wc = win[cidx];
+                    const int v = var_index[cidx];
+                    PushRun pr{};
+                    if (ic.kind == DFD_COL_FIXED) {
+                        pr.kind = RUN_BYTES; pr.src = (const char*)wc.values + (size_t)seg * ic.width;
+                        pr.dst = ob + o_val[cidx] + (size_t)drow * ic.width; pr.n = cnt * ic.width;
+                        runs.push_back(pr);
+                    } else if (ic.kind == DFD_COL_BOOL) {
+                        bit_run((const char*)wc.values, seg, o_bits[cidx], sh0 + drow, cnt);
+                    } else {
+                        // entries 1..cnt of the segment's offsets are the ends of its rows: re-based onto the dense bytes
+                        const int ow = ic.kind == DFD_COL_LARGE_UTF8 ? 8 : 4;
+                        const size_t b = (size_t)v * NS + sg;
+                        pr.kind = ow == 8 ? RUN_OFF64 : RUN_OFF32; pr.src = (const char*)wc.offsets + (size_t)(seg + 1) * ow;
+                        pr.dst = ob + o_off[cidx] + (size_t)drow * ow; pr.n = cnt; pr.a = bseg[b]; pr.b = out_bytes[v] + dbytes[v];
+                        runs.push_back(pr);
+                        if (bcnt[b] > 0) {
+                            PushRun br{};
+                            br.kind = RUN_BYTES; br.src = (const char*)wc.values + bseg[b]; br.dst = ob + o_val[cidx] + dbytes[v]; br.n = bcnt[b];
+                            runs.push_back(br);
+                            dbytes[v] += bcnt[b];
+                        }
+                    }
+                    if (wc.validity) bit_run((const char*)wc.validity, seg, o_valid[cidx], sh0 + drow, cnt);
+                }
+                drow += cnt;
+            }
+            // the host word this chunk shares with the last one: fold in that chunk's bits below out_row
+            if (sh0 && last >= 0)
+                for (size_t l = 0; l < lanes.size(); ++l)
+                    bit_run((const char*)x->out_stage[last].ptr + lane_off[last][l], ((out_row >> 5) - last_word) * 32, lanes[l], 0, sh0);
+            int blocks = 0, bblocks = 0;
+            for (PushRun& r : runs) { r.first_block = blocks; blocks += (int)((push_run_out_bytes(r) + PUSH_CHUNK - 1) / PUSH_CHUNK); }
+            for (BitRun& r : bruns) { r.first_block = bblocks; bblocks += (int)((bit_run_words(r) + BIT_WORDS_PER_CTA - 1) / BIT_WORDS_PER_CTA); }
+            // (the previous chunk's run upload has completed: push_shuffle_locked synchronised the stream since)
+            const size_t run_bytes = (runs.size() * sizeof(PushRun) + 15) / 16 * 16, need = run_bytes + bruns.size() * sizeof(BitRun);
+            if (need > x->cruns_cap) {
+                cudaFree(x->d_cruns); cudaFreeHost(x->h_cruns);
+                x->d_cruns = nullptr; x->h_cruns = nullptr; x->cruns_cap = 0;
+                CUDA_TRY(cudaMalloc(&x->d_cruns, need * 2), "cudaMalloc(compaction runs)");
+                CUDA_TRY(cudaHostAlloc(&x->h_cruns, need * 2, cudaHostAllocPortable), "cudaHostAlloc(compaction runs)");
+                x->cruns_cap = need * 2;
+            }
+            memcpy(x->h_cruns, runs.data(), runs.size() * sizeof(PushRun));
+            memcpy((char*)x->h_cruns + run_bytes, bruns.data(), bruns.size() * sizeof(BitRun));
+            CUDA_TRY(cudaMemcpyAsync(x->d_cruns, x->h_cruns, need, cudaMemcpyHostToDevice, s), "H2D compaction runs");
+            if (!runs.empty()) {
+                k_push_runs<<<(unsigned)blocks, PUSH_THREADS, 0, s>>>((const PushRun*)x->d_cruns, (int)runs.size());
+                CUDA_TRY(cudaGetLastError(), "k_push_runs");
+                c->metrics.kernel_launches++;
+            }
+            if (!bruns.empty()) {
+                k_place_bits<<<(unsigned)bblocks, PUSH_THREADS, 0, s>>>((const BitRun*)((char*)x->d_cruns + run_bytes), (int)bruns.size());
+                CUDA_TRY(cudaGetLastError(), "k_place_bits");
+                c->metrics.kernel_launches++;
+            }
+            CUDA_TRY(cudaEventRecord(x->e_out[cur], s), "record");
+            // ---- D2H of the dense chunk
+            CUDA_TRY(cudaStreamWaitEvent(x->s_d2h, x->e_out[cur], 0), "wait");
+            for (int cidx = 0; cidx < n_cols; ++cidx) {
+                const dfd_column& ic = in_cols[cidx];
+                const dfd_column& oc = out_cols[cidx];
+                const int v = var_index[cidx];
+                if (ic.kind == DFD_COL_FIXED) {
+                    CUDA_TRY(cudaMemcpyAsync((char*)oc.values + (size_t)out_row * ic.width, ob + o_val[cidx], (size_t)got * ic.width,
+                                             cudaMemcpyDeviceToHost, x->s_d2h), "D2H");
+                } else if (ic.kind == DFD_COL_BOOL) {
+                    CUDA_TRY(cudaMemcpyAsync((char*)oc.values + (size_t)(out_row >> 5) * 4, ob + o_bits[cidx], (size_t)nw * 4, cudaMemcpyDeviceToHost,
+                                             x->s_d2h), "D2H");
+                } else {
+                    const size_t ow = ic.kind == DFD_COL_LARGE_UTF8 ? 8 : 4;
+                    CUDA_TRY(cudaMemcpyAsync((char*)oc.offsets + (size_t)(out_row + 1) * ow, ob + o_off[cidx], (size_t)got * ow, cudaMemcpyDeviceToHost,
+                                             x->s_d2h), "D2H");
+                    if (chunk_bytes[v])
+                        CUDA_TRY(cudaMemcpyAsync((char*)oc.values + out_bytes[v], ob + o_val[cidx], (size_t)chunk_bytes[v], cudaMemcpyDeviceToHost,
+                                                 x->s_d2h), "D2H");
+                }
+                if (win[cidx].validity)
+                    CUDA_TRY(cudaMemcpyAsync((char*)oc.validity + (size_t)(out_row >> 5) * 4, ob + o_valid[cidx], (size_t)nw * 4, cudaMemcpyDeviceToHost,
+                                             x->s_d2h), "D2H");
+            }
+            CUDA_TRY(cudaEventRecord(x->e_d2h[cur], x->s_d2h), "record");
+            stage_used[cur] = true;
+            last = cur;
+            last_word = out_row >> 5;
+        }
+        out_row += got;
+        for (int v = 0; v < V; ++v) out_bytes[v] += chunk_bytes[v];
+    }
+    if (out_row == 0) first_offsets();
+    return DFD_OK;
+}
+
 /* Host-to-host shuffle (the end-to-end path of the multi-worker exchange): this worker's rows live in
  * HOST column buffers, its received destinations are delivered into HOST (ideally pinned) buffers.
  * The rows are cut into `n_chunks` equal pieces (every worker must pass the same n_chunks: each chunk
- * is one collective fused shuffle) and pipelined: H2D of chunk i+1 and D2H of chunk i-1 overlap the
- * shuffle of chunk i (two input stages, two receive-window slots).  Output: chunk-major — chunk i's
+ * is one collective shuffle) and pipelined: H2D of chunk i+1 and D2H of chunk i-1 overlap the
+ * shuffle of chunk i.  Fixed-width non-null schemas take the two-pass fused transport (two input
+ * stages, two receive-window slots); any nullable, Boolean or string column sends the whole schema
+ * through the push transport (host_push_chunks_locked).  Output: chunk-major — chunk i's
  * destination q occupies rows [chunk_part_starts[i*(P+1)+q], chunk_part_starts[i*(P+1)+q+1]) of
  * every out column (absolute row offsets), exactly like a stream of per-destination record batches. */
 int dfd_shuffle_host(dfd_exchange* x, dfd_partitioner* part, const dfd_column* in_cols, int n_cols, int64_t n_rows,
@@ -1327,14 +1728,20 @@ int dfd_shuffle_host(dfd_exchange* x, dfd_partitioner* part, const dfd_column* i
     if (!x || !part || !in_cols || !out_cols || !chunk_part_starts || n_chunks < 1 || n_rows < 0)
         return set_error(DFD_ERR_INVALID_ARGUMENT, "dfd_shuffle_host: bad arguments");
     const uint32_t P = partitions_per_task;
-    for (int i = 0; i < n_cols; ++i)
-        if (in_cols[i].kind != DFD_COL_FIXED || in_cols[i].validity || in_cols[i].offset != 0 || out_cols[i].kind != DFD_COL_FIXED ||
-            out_cols[i].width != in_cols[i].width || !in_cols[i].values || !out_cols[i].values)
-            return set_error(DFD_ERR_UNSUPPORTED, "column %d: dfd_shuffle_host moves fixed-width non-null columns", i);
+    const bool push = host_shuffle_needs_push(in_cols, out_cols, n_cols);
+    if (push) {
+        int rc = check_host_push_columns(in_cols, out_cols, n_cols, n_rows);
+        if (rc) return rc;
+    } else {
+        for (int i = 0; i < n_cols; ++i)
+            if (in_cols[i].kind != DFD_COL_FIXED || in_cols[i].validity || in_cols[i].offset != 0 || out_cols[i].kind != DFD_COL_FIXED ||
+                out_cols[i].width != in_cols[i].width || !in_cols[i].values || !out_cols[i].values)
+                return set_error(DFD_ERR_UNSUPPORTED, "column %d: dfd_shuffle_host moves fixed-width non-null columns", i);
+    }
     std::unique_lock<std::mutex> lk;
     int rc = begin_shuffle(x, part, in_cols, out_cols, P, "dfd_shuffle_host", lk);
     if (rc) return rc;
-    x->shuffles += (uint64_t)n_chunks - 1;  // one collective fused shuffle per chunk
+    x->shuffles += (uint64_t)n_chunks - 1;  // one collective shuffle per chunk
     dfd_ctx* c = x->ctx;
     if (!x->s_h2d) {
         CUDA_TRY(cudaStreamCreateWithFlags(&x->s_h2d, cudaStreamNonBlocking), "stream");
@@ -1343,7 +1750,18 @@ int dfd_shuffle_host(dfd_exchange* x, dfd_partitioner* part, const dfd_column* i
             CUDA_TRY(cudaEventCreateWithFlags(&x->e_h2d[i], cudaEventDisableTiming), "event");
             CUDA_TRY(cudaEventCreateWithFlags(&x->e_k[i], cudaEventDisableTiming), "event");
             CUDA_TRY(cudaEventCreateWithFlags(&x->e_d2h[i], cudaEventDisableTiming), "event");
+            CUDA_TRY(cudaEventCreateWithFlags(&x->e_out[i], cudaEventDisableTiming), "event");
         }
+    }
+    if (push) {
+        rc = host_push_chunks_locked(x, part, in_cols, n_cols, n_rows, P, n_chunks, out_cols, out_capacity_rows, chunk_part_starts);
+        x->pending.kind = dfd_exchange::Pending::NONE;
+        // whether or not every chunk went through, no copy may touch the caller's buffers once the call has returned
+        const cudaError_t e1 = cudaStreamSynchronize(x->s_h2d), e2 = cudaStreamSynchronize(c->stream), e3 = cudaStreamSynchronize(x->s_d2h);
+        if (rc) return rc;
+        for (cudaError_t e : {e1, e2, e3})
+            if (e != cudaSuccess) return cuda_error(e, "dfd_shuffle_host");
+        return DFD_OK;
     }
     const int64_t max_chunk = (n_rows + n_chunks - 1) / n_chunks + 1;
     std::vector<size_t> col_off(n_cols);

@@ -306,7 +306,14 @@ class NetworkShuffleExec:
     def shuffle_host(self, exchange: ShuffleExchange, host_in: Sequence[DeviceColumn], n_rows: int, n_chunks: int,
                      host_out: Sequence[DeviceColumn], out_capacity_rows: int) -> np.ndarray:
         """Host-to-host pipelined shuffle (`dfd_shuffle_host`): `host_in` / `host_out` describe HOST (pinned)
-        column buffers.  Returns chunk_part_starts[n_chunks][P+1] (absolute row offsets into host_out)."""
+        column buffers.  Returns chunk_part_starts[n_chunks][P+1] (absolute row offsets into host_out).
+
+        Every column kind moves.  A fixed-width non-null schema takes the two-pass fused transport (two window slots);
+        a schema with a nullable, Boolean, Utf8, LargeUtf8 or Binary column takes the push transport (the whole window
+        per chunk).  A column is nullable when `host_out[i].validity` is set (the schema's flag: every worker must agree)
+        or `host_in[i]` has a bitmap.  String outputs need offsets of `out_capacity_rows + 1` entries and `values_bytes`
+        of byte capacity: the offsets start at 0 and index one dense byte buffer across all chunks.  Bitmaps are written
+        in whole 32-bit words, so size them (out_capacity_rows + 31) // 32 * 4 bytes.  Inputs must be at offset 0."""
         P = self.properties.partition_count
         starts = (C.c_int64 * (n_chunks * (P + 1)))()
         nv.check(nv.lib().dfd_shuffle_host(exchange._h, self._partitioner(exchange), columns_to_c(host_in), len(host_in), n_rows, P, n_chunks,

@@ -641,14 +641,34 @@ uint32_t dfd_exchange_pending_segments(const dfd_exchange* x);
 
 /* Host-to-host collective shuffle (end-to-end path of the multi-worker exchange; replaces, per
  * worker, "execute the producer plan, Flight-encode, stream, decode" of
- * src/worker/impl_execute_task.rs:36-169 + src/worker/worker_connection_pool.rs:143-390 for
- * fixed-width non-null columns).  HOST in_cols (n_rows) -> HOST out_cols (out_capacity_rows;
- * pinned memory from dfd_host_alloc gives full PCIe rate).  The rows are cut into n_chunks
- * equal pieces — one fused collective shuffle each, so every worker must pass the same
- * n_chunks — and H2D(i+1) | shuffle(i) | D2H(i-1) overlap (needs a receive window of
- * at least 2 x the per-chunk receive size).  Output is chunk-major, like a stream of
- * per-destination batches: chunk i / local partition q = rows
- * [chunk_part_starts[i*(P+1)+q], chunk_part_starts[i*(P+1)+q+1]) of every out column. */
+ * src/worker/impl_execute_task.rs:36-169 + src/worker/worker_connection_pool.rs:143-390).
+ * HOST in_cols (n_rows) -> HOST out_cols (out_capacity_rows; pinned memory from dfd_host_alloc
+ * gives full PCIe rate).  The rows are cut into n_chunks equal pieces — one collective shuffle
+ * each, so every worker must pass the same n_chunks; dfd_exchange_stats counts one shuffle per
+ * chunk — and H2D(i+1) | shuffle(i) | D2H(i-1) overlap.  Output is chunk-major, like a stream
+ * of per-destination batches: chunk i / local partition q = rows
+ * [chunk_part_starts[i*(P+1)+q], chunk_part_starts[i*(P+1)+q+1]) of every out column, the
+ * producers' rows in task order.  Every input has Arrow offset 0 and fixed widths are 1/2/4/8/16
+ * bytes (else DFD_ERR_UNSUPPORTED, before any communication).
+ * The SCHEMA picks the transport, so every worker takes the same one:
+ *   - all columns fixed-width and non-null: the two-pass fused transport through two halves of
+ *     the receive window (needs a window of at least 2 x the per-chunk receive size);
+ *   - any column nullable (out_cols[c].validity != NULL on entry, or an input bitmap), Boolean,
+ *     Utf8, LargeUtf8 or Binary: the push transport (as dfd_shuffle_device_onepass), which takes
+ *     the whole window per chunk.  A chunk that some worker's window cannot hold is
+ *     DFD_ERR_CAPACITY on every worker, with nothing of that chunk written.  The chunk's window
+ *     segments are compacted on the device into one dense chunk and copied out:
+ *       Utf8 / LargeUtf8 / Binary outputs take offsets of out_capacity_rows + 1 entries and
+ *       `values` of values_bytes bytes: the offsets start at 0 and index one dense byte buffer
+ *       across all chunks;
+ *       bitmaps (validity, Boolean values): the 32-bit words covering rows [0, total) are written,
+ *       the bits at and past total are zero and nothing past those words is written (size them
+ *       as (out_capacity_rows + 31) / 32 * 4 bytes);
+ *       a worker whose rows, string bytes or Utf8 / Binary offsets past INT32_MAX do not fit
+ *       returns DFD_ERR_CAPACITY naming what it needed, with the chunks before that one
+ *       delivered; its peers then return an error (a flag wait of their next chunk times out
+ *       after a bounded time) instead of hanging.
+ * No shuffle is left pending afterwards (dfd_exchange_collect has nothing to report). */
 int dfd_shuffle_host(dfd_exchange* x, dfd_partitioner* p, const dfd_column* in_cols, int n_cols, int64_t n_rows,
                      uint32_t partitions_per_task, int n_chunks, const dfd_column* out_cols,
                      int64_t out_capacity_rows, int64_t* chunk_part_starts);
