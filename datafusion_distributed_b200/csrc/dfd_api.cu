@@ -132,6 +132,7 @@ int dfd::PartitionJob::prepare(Partitioner* part, const dfd_column* in_cols, int
     passes.clear();
     var_cols.clear();
     gathers.clear();
+    bit_gathers.clear();
     d_src = nullptr;
     bytes = 0;
     Ctx* c = p->ctx;
@@ -156,6 +157,11 @@ int dfd::PartitionJob::prepare(Partitioner* part, const dfd_column* in_cols, int
             if (ic.width < 1) return set_error(DFD_ERR_UNSUPPORTED, "column %d: fixed width %d < 1", i, ic.width);
             gathers.push_back(GatherCol{ic.values, oc.values, ic.offset, ic.width});
             bytes += (uint64_t)n_rows * ic.width;
+        } else if (ic.kind == COL_BIT_ROWS && p->bit_rows && !peer) {
+            if (ic.width < 1) return set_error(DFD_ERR_UNSUPPORTED, "column %d: bit rows of %d bits", i, ic.width);
+            if ((uintptr_t)oc.values & 3) return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: output bit rows must be 4-byte aligned", i);
+            bit_gathers.push_back(GatherCol{ic.values, oc.values, ic.offset, ic.width});
+            bytes += (uint64_t)(n_rows * ic.width + 7) / 8;
         } else if (ic.kind == DFD_COL_FIXED) {
             if (((uintptr_t)ic.values | (uintptr_t)oc.values) & (uintptr_t)(ic.width - 1))
                 return set_error(DFD_ERR_INVALID_ARGUMENT, "column %d: buffers must be aligned to the value width", i);
@@ -224,7 +230,7 @@ int dfd::PartitionJob::prepare(Partitioner* part, const dfd_column* in_cols, int
                 if (e != cudaSuccess) return cuda_error(e, "cudaMemsetAsync(bit-packed output)");
             }
     }
-    if ((!var_cols.empty() || !gathers.empty()) && n_rows > 0) {
+    if ((!var_cols.empty() || !gathers.empty() || !bit_gathers.empty()) && n_rows > 0) {
         // K4 and the gathers need the input row of every output row: scatter an iota column with the rest
         const size_t nb = (((size_t)n_rows * 4) + 255) & ~(size_t)255;
         const int64_t n_blocks = (n_rows + VAR_BLOCK * VAR_ITEMS - 1) / (VAR_BLOCK * VAR_ITEMS);
@@ -370,7 +376,7 @@ int dfd::PartitionJob::run_scatter(const int64_t* dest_base, void* const* peer_b
         sp.dest_cache = d_dest_cache;
         if ((rc = launch_width_groups(sp, passes, ScatterKind::TwoPass, &launches))) return rc;
     }
-    if (!gathers.empty()) {
+    if (!gathers.empty() || !bit_gathers.empty()) {
         int rc = run_gathers();
         if (rc) return rc;
     }
@@ -471,12 +477,18 @@ static int launch_varwidth(const dfd::PartitionJob::VarCol& vc, const uint32_t* 
     return DFD_OK;
 }
 
-// One k_gather_rows launch per gathered column (none for 0 rows); counted as kernel launches, not scatter launches.
+// One k_gather_rows / k_gather_bit_rows launch per gathered column (none for 0 rows); counted as kernel launches, not
+// scatter launches.
 int dfd::PartitionJob::run_gathers() {
     if (n_rows == 0) return DFD_OK;
     Ctx* c = p->ctx;
     for (const GatherCol& g : gathers) {
         int rc = launch_gather_rows(g.in, g.in_offset, d_src, n_rows, g.width, g.out, c->sm_count, stream);
+        if (rc) return rc;
+        c->metrics.kernel_launches++;
+    }
+    for (const GatherCol& g : bit_gathers) {
+        int rc = launch_gather_bit_rows(g.in, g.in_offset, d_src, n_rows, g.width, g.out, c->sm_count, stream);
         if (rc) return rc;
         c->metrics.kernel_launches++;
     }

@@ -54,6 +54,11 @@ struct FieldInfo {
     int64_t child_flags = 0;
     int32_t child_width = 0;       // list child: 0 = Utf8 / Binary (offsets + bytes), > 0 = fixed-width primitive of that many bytes
     bool nodev() const { return list; }
+    // FixedSizeList<T, n> payload (n = fsl_n): the field is the device column of its rows and carries the list's validity.
+    // Its values are the child's, n x child_width bytes per row (kind FIXED), or for a Boolean child (child_width 0) n bits
+    // per row (kind COL_BIT_ROWS).  A nullable child adds one hidden COL_BIT_ROWS column (h_valid): its validity, n bits per row.
+    bool fsl = false;
+    int32_t fsl_n = 0;
     bool dict = false;             // dictionary-encoded: `format` is the index type, dict_* describe the values
     bool dict_index_unsigned = false;  // UInt8/16/32/64 indices ("C" "S" "I" "L")
     std::string dict_format;
@@ -253,6 +258,7 @@ struct PinnedPool : std::enable_shared_from_this<PinnedPool> {
 
     static size_t value_bytes(const FieldInfo& f, int64_t rows) {
         if (f.var()) return 0;  // string bytes are sized per chunk
+        if (f.kind == COL_BIT_ROWS) return bitmap_bytes(rows * f.width);
         return f.kind == DFD_COL_BOOL ? (size_t)((rows + 63) / 64 * 8 + 8) : (size_t)rows * (size_t)f.width;
     }
     static size_t bitmap_bytes(int64_t rows) { return (size_t)((rows + 63) / 64 * 8 + 8); }
@@ -446,7 +452,7 @@ int export_schema(const std::vector<FieldInfo>& fields, ArrowSchema* out) {
         c.name = p->fields[i].name.c_str();
         c.flags = p->fields[i].flags;
         c.release = schema_child_release;
-        if (p->fields[i].list) {
+        if (p->fields[i].list || p->fields[i].fsl) {
             ArrowSchema& it = p->items[i];
             memset(&it, 0, sizeof it);
             it.format = p->fields[i].child_format.c_str();
@@ -688,6 +694,31 @@ int emit_slot(dfd_repartition_exec* x, Slot& s) {
                 bp->child_ptrs[c] = &a;
                 continue;
             }
+            if (f.fsl) {
+                // FixedSizeList: a zero-copy slice of the parent (its validity) over the chunk-wide child, whose element
+                // (start + i) x n starts row i of the slice
+                bp->child_bufs[4 * c] = hv ? oc->validity[c] : nullptr;
+                ArrowArray& g = bp->grand[c];
+                memset(&g, 0, sizeof g);
+                bp->grand_bufs[3 * c] = f.h_valid >= 0 ? oc->values[(size_t)f.h_valid] : nullptr;
+                bp->grand_bufs[3 * c + 1] = oc->values[c];
+                g.length = s.rows * f.fsl_n;
+                g.null_count = f.h_valid >= 0 ? -1 : 0;
+                g.n_buffers = 2;
+                g.buffers = &bp->grand_bufs[3 * c];
+                g.release = child_release;
+                bp->grand_ptrs[c] = &g;
+                a.length = cnt;
+                a.offset = start;
+                a.null_count = hv ? -1 : 0;
+                a.n_buffers = 1;
+                a.buffers = &bp->child_bufs[4 * c];
+                a.n_children = 1;
+                a.children = &bp->grand_ptrs[c];
+                a.release = child_release;
+                bp->child_ptrs[c] = &a;
+                continue;
+            }
             const bool var = f.var();
             bp->child_bufs[4 * c] = hv ? oc->validity[c] : nullptr;
             bp->child_bufs[4 * c + 1] = f.view ? oc->views[c] : (var ? oc->offsets[c] : oc->values[c]);
@@ -824,9 +855,10 @@ int flush_current(dfd_repartition_exec* x) {
             XCUDA(x, cudaMemcpyAsync(sc.d_in_valid, sc.h_valid, bm, cudaMemcpyHostToDevice, x->s_h2d), "H2D validity");
             x->bytes_h2d += bm;
         }
-        if (f.kind == DFD_COL_BOOL) {
-            XCUDA(x, cudaMemcpyAsync(sc.d_in, sc.h_bool, bm, cudaMemcpyHostToDevice, x->s_h2d), "H2D boolean values");
-            x->bytes_h2d += bm;
+        if (f.kind == DFD_COL_BOOL || f.kind == COL_BIT_ROWS) {
+            const size_t nb = f.kind == DFD_COL_BOOL ? bm : (size_t)((s.rows * f.width + 7) / 8);
+            XCUDA(x, cudaMemcpyAsync(sc.d_in, sc.h_bool, nb, cudaMemcpyHostToDevice, x->s_h2d), "H2D boolean values");
+            x->bytes_h2d += nb;
         }
         if (f.var()) {
             XCUDA(x, cudaMemcpyAsync(sc.d_in_off, sc.h_off, (size_t)(s.rows + 1) * f.ow(), cudaMemcpyHostToDevice, x->s_h2d), "H2D offsets");
@@ -938,6 +970,7 @@ int flush_current(dfd_repartition_exec* x) {
         const FieldInfo& f = x->fields[i];
         const SlotCol& sc = s.col[i];
         size_t nb = f.kind == DFD_COL_BOOL ? (size_t)((s.rows + 7) / 8) : (size_t)s.rows * f.width;
+        if (f.kind == COL_BIT_ROWS) nb = (size_t)((s.rows * f.width + 31) / 32) * 4;  // (whole words, as the gather wrote them)
         const void* src = sc.d_out;
         if (f.var()) {
             nb = (size_t)sc.data_bytes;
@@ -1188,8 +1221,10 @@ int prepare_rows(dfd_repartition_exec* x, const ArrowArray* b, const HeldInput& 
         const ArrowArray* c = b->children[i];
         if (validity_of(c) && !(f.flags & ARROW_FLAG_NULLABLE) && c->null_count > 0)
             return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": nulls in a column the schema declares non-nullable");
-        if (f.list && (c->n_children != 1 || !c->children[0]))
+        if ((f.list || f.fsl) && (c->n_children != 1 || !c->children[0]))
             return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": list array without a child");
+        if (f.fsl && validity_of(c->children[0]) && !(f.child_flags & ARROW_FLAG_NULLABLE) && c->children[0]->null_count > 0)
+            return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": nulls in a list child the schema declares non-nullable");
         if (!f.dict) continue;
         if (!c->dictionary) return fail(x, DFD_ERR_INVALID_ARGUMENT, "column " + f.name + ": dictionary array without a dictionary");
         // one dictionary per chunk (it travels by reference).  A batch whose dictionary is a different OBJECT with the same
@@ -1260,8 +1295,8 @@ int stage_rows_host(dfd_repartition_exec* x, const ArrowArray* b, const HeldInpu
     Slot& s = x->slots[x->cur];
     std::lock_guard<std::mutex> lk(x->ctx->mu);
     XCUDA(x, cudaSetDevice(x->ctx->device), "cudaSetDevice");
-    auto host_bitmap = [&](uint8_t*& p) -> uint8_t* {
-        if (!p && cudaHostAlloc((void**)&p, PinnedPool::bitmap_bytes(x->chunk_rows) + 8, cudaHostAllocPortable) != cudaSuccess) p = nullptr;
+    auto host_bitmap = [&](uint8_t*& p, int64_t bits_per_row = 1) -> uint8_t* {
+        if (!p && cudaHostAlloc((void**)&p, PinnedPool::bitmap_bytes(x->chunk_rows * bits_per_row) + 8, cudaHostAllocPortable) != cudaSuccess) p = nullptr;
         return p;
     };
     auto stage_validity = [&](size_t i, const uint8_t* valid, int64_t lo) -> int {
@@ -1334,6 +1369,28 @@ int stage_rows_host(dfd_repartition_exec* x, const ArrowArray* b, const HeldInpu
             if ((rc2 = stage_var((size_t)f.h_len, tl.off.data(), tl.bytes.data())) || (rc2 = stage_var((size_t)f.h_bytes, tb.off.data(), child_bytes))) return rc2;
             if (f.h_valid >= 0 && (rc2 = stage_var((size_t)f.h_valid, ov32, dvb))) return rc2;
             if ((rc2 = stage_validity((size_t)f.h_len, valid, lo))) return rc2;  // the list's own validity rides on the lengths column
+            continue;
+        }
+        if (f.fsl) {
+            // FixedSizeList: the child values of the rows go to the device straight from the batch; bit rows (Boolean values,
+            // child validity) are concatenated on the host like any bitmap, n bits per row
+            const ArrowArray* v = c->children[0];
+            const dfd::host::FslSpan sp = dfd::host::fsl_span(v->offset, lo, n, f.fsl_n, f.child_width);
+            auto bit_rows = [&](size_t h, const uint8_t* src) -> int {
+                uint8_t* hb = host_bitmap(s.col[h].h_bool, f.fsl_n);
+                if (!hb) return fail(x, DFD_ERR_OOM, "pinned host allocation failed");
+                append_bits(hb, s.rows * f.fsl_n, src, sp.first_bit, sp.n_bits);
+                return DFD_OK;
+            };
+            if (f.kind == DFD_COL_FIXED) {
+                if (sp.n_bytes) XCUDA(x, cudaMemcpyAsync((char*)s.col[i].d_in + (size_t)s.rows * f.width, (const char*)v->buffers[1] + sp.first_byte, sp.n_bytes,
+                                                         cudaMemcpyHostToDevice, x->s_h2d), "H2D");
+                x->bytes_h2d += sp.n_bytes;
+            } else if ((rc2 = bit_rows(i, (const uint8_t*)v->buffers[1]))) {
+                return rc2;
+            }
+            if (f.h_valid >= 0 && (rc2 = bit_rows((size_t)f.h_valid, validity_of(v)))) return rc2;  // (no bitmap: all valid)
+            if ((rc2 = stage_validity(i, valid, lo))) return rc2;
             continue;
         }
         if (f.dict && x->key_of_field[i] >= 0 && s.rows == 0) {
@@ -1453,6 +1510,33 @@ int stage_rows_device(dfd_repartition_exec* x, const ArrowArray* b, const HeldIn
                 bytes(hv, vb);
             }
             validity(hl, valid, lo);  // the list's own validity rides on the lengths column
+            continue;
+        }
+        if (f.fsl) {
+            // FixedSizeList: one copy of the rows' child values, or bitmap appends of n bits per row (Boolean values, child validity)
+            const ArrowArray* v = c->children[0];
+            const dfd::host::FslSpan sp = dfd::host::fsl_span(v->offset, lo, n, f.fsl_n, f.child_width);
+            auto bit_rows = [&](size_t h, const void* src) {
+                StageJob bj;
+                bj.op = STAGE_BITS;
+                bj.src = src;
+                bj.a = sp.first_bit;
+                bj.dst = s.col[h].d_in;
+                bj.b = bj.c = s.rows * f.fsl_n;
+                bj.n = sp.n_bits;
+                jobs.push_back(bj);
+            };
+            if (f.kind == DFD_COL_FIXED) {
+                StageJob cp;
+                cp.src = (const char*)v->buffers[1] + sp.first_byte;
+                cp.dst = (char*)s.col[i].d_in + (size_t)s.rows * f.width;
+                cp.n = (int64_t)sp.n_bytes;
+                jobs.push_back(cp);
+            } else {
+                bit_rows(i, v->buffers[1]);
+            }
+            if (f.h_valid >= 0) bit_rows((size_t)f.h_valid, validity_of(v));  // (no bitmap: all valid)
+            validity(i, valid, lo);
             continue;
         }
         if (f.dict && x->key_of_field[i] >= 0 && s.rows == 0) {
@@ -1788,6 +1872,27 @@ int pull_stream(dfd_repartition_exec* x, Stream* input, int (*push)(dfd_repartit
 }
 }  // namespace
 
+// The chunk size of an operator created with chunk_rows = 0: 4 Mi rows, or, for a schema with a FixedSizeList column (whose
+// rows can be kilobytes: an embedding), the largest multiple of 64 rows up to that whose fixed-width buffers (values, bit
+// rows, bitmaps) fit FSL_CHUNK_BUDGET — what cfg-2's 4 Mi rows x 64 B hold.  Each of the pipeline's in-slots, out-slots and
+// output chunks holds one such chunk.
+constexpr int64_t DEFAULT_CHUNK_ROWS = 4 << 20;
+constexpr int64_t FSL_CHUNK_BUDGET = (int64_t)256 << 20;
+
+static int64_t default_chunk_rows(const std::vector<FieldInfo>& fields) {
+    bool fsl = false;
+    int64_t bits = 0;  // fixed-width bits per row
+    for (const FieldInfo& f : fields) {
+        fsl |= f.fsl;
+        if (f.nodev() || f.var()) continue;
+        bits += f.kind == DFD_COL_BOOL ? 1 : f.kind == COL_BIT_ROWS ? f.width : 8 * (int64_t)f.width;
+        if (f.flags & ARROW_FLAG_NULLABLE) bits += 1;
+    }
+    if (!fsl || bits == 0) return DEFAULT_CHUNK_ROWS;
+    const int64_t rows = FSL_CHUNK_BUDGET * 8 / bits / 64 * 64;
+    return rows < 64 ? 64 : rows > DEFAULT_CHUNK_ROWS ? DEFAULT_CHUNK_ROWS : rows;
+}
+
 extern "C" {
 
 int dfd_arrow_format_layout(const char* format, int32_t* kind, int32_t* width) {
@@ -1813,6 +1918,34 @@ static bool list_child_ok(const ArrowSchema* c, int32_t* child_width) {
     return true;
 }
 
+// FixedSizeList<T, n> ("+w:n", n >= 1) payload: the child is a Boolean or a fixed-width primitive that list_child_ok takes.
+// Fills `f` (0 = the column is not a FixedSizeList), or refuses it naming the column.
+static int fixed_size_list_child(const ArrowSchema* c, long long i, bool is_key, FieldInfo* f) {
+    const char* name = c->name ? c->name : "";
+    if (!c->format || strncmp(c->format, "+w:", 3) != 0) return DFD_OK;
+    if (is_key) return set_error(DFD_ERR_UNSUPPORTED, "column %lld (%s): FixedSizeList columns cannot be hash keys", i, name);
+    char* end = nullptr;
+    const long long n = strtoll(c->format + 3, &end, 10);
+    if (end == c->format + 3 || *end || n < 1)
+        return set_error(DFD_ERR_UNSUPPORTED, "column %lld (%s): FixedSizeList format '%s' is not supported (n >= 1)", i, name, c->format);
+    const ArrowSchema* v = c->n_children == 1 && c->children ? c->children[0] : nullptr;
+    int32_t k = 0, w = 0;
+    if (!v || !v->format || c->dictionary || v->dictionary || v->n_children != 0 || !parse_format(v->format, &k, &w) ||
+        !(k == DFD_COL_BOOL || (k == DFD_COL_FIXED && v->format[0] != 'w')))
+        return set_error(DFD_ERR_UNSUPPORTED, "column %lld (%s): FixedSizeList child type '%s' is not supported (fixed-width primitives and Boolean only)", i,
+                         name, v && v->format ? v->format : "(none)");
+    if (n * (w ? w : 1) > 0x7fffffffLL) return set_error(DFD_ERR_UNSUPPORTED, "column %lld (%s): FixedSizeList rows of more than 2 GiB", i, name);
+    f->fsl = true;
+    f->fsl_n = (int32_t)n;
+    f->child_width = w;
+    f->kind = k == DFD_COL_BOOL ? COL_BIT_ROWS : DFD_COL_FIXED;
+    f->width = k == DFD_COL_BOOL ? (int32_t)n : (int32_t)(n * w);
+    f->child_name = v->name ? v->name : "item";
+    f->child_format = v->format;
+    f->child_flags = v->flags;
+    return DFD_OK;
+}
+
 // One column `i` of the record-batch schema: can the operator move it, and — if it is a hash key — hash it like DataFusion?
 // Fills `f` with what the operator keeps of it.
 static int describe_column(const ArrowSchema* c, long long i, bool is_key, FieldInfo* f) {
@@ -1830,6 +1963,8 @@ static int describe_column(const ArrowSchema* c, long long i, bool is_key, Field
         f->child_flags = c->children[0]->flags;
         return DFD_OK;
     }
+    if (int rc = fixed_size_list_child(c, i, is_key, f)) return rc;
+    if (f->fsl) return DFD_OK;
     if (!c->format || !parse_format(c->format, &f->kind, &f->width))
         return set_error(DFD_ERR_UNSUPPORTED, "column %lld (%s): Arrow format '%s' is not supported", i, name, c->format ? c->format : "(null)");
     f->view = c->format[0] == 'v';
@@ -1910,6 +2045,18 @@ int dfd_repartition_exec_create(dfd_ctx* ctx, const struct ArrowSchema* schema, 
     // hidden device columns of the list fields, appended after the visible ones
     x->n_visible = x->fields.size();
     for (size_t i = 0; i < x->n_visible; ++i) {
+        if (x->fields[i].fsl && (x->fields[i].child_flags & ARROW_FLAG_NULLABLE)) {  // the child's validity: n bits per row
+            FieldInfo h;
+            h.name = x->fields[i].name + ".validity";
+            h.format = x->fields[i].format;
+            h.kind = COL_BIT_ROWS;
+            h.width = x->fields[i].fsl_n;
+            h.hidden = true;
+            h.role = 3;
+            x->key_of_field.push_back(-1);
+            x->fields.push_back(h);
+            x->fields[i].h_valid = (int)x->fields.size() - 1;
+        }
         if (!x->fields[i].list) continue;
         auto hidden = [&](const char* tag, bool nullable) {
             FieldInfo h;
@@ -1938,6 +2085,7 @@ int dfd_repartition_exec_create(dfd_ctx* ctx, const struct ArrowSchema* schema, 
     for (int k = 0; k < n_keys; ++k) dev_keys[k] = dev_pos[(size_t)key_cols[k]];  // keys address the compact device column list
     int rc = dfd_partitioner_create(ctx, num_partitions, dev_keys.data(), n_keys, nullptr, &x->part);
     if (rc) return rc;  // (x has no CUDA resources yet; unique_ptr frees it)
+    x->part->bit_rows = true;  // (FixedSizeList bit rows)
     for (int k = 0; k < n_keys; ++k) {  // interval keys hash field by field (arrow's derived Hash), not as one integer
         const int mode = interval_key_mode(x->fields[(size_t)key_cols[k]].format);  // (a dictionary field's format is its index type)
         if (mode != DFD_KEY_HASH_PLAIN && (rc = dfd_partitioner_set_key_hash_mode(x->part, k, mode))) {
@@ -1946,7 +2094,7 @@ int dfd_repartition_exec_create(dfd_ctx* ctx, const struct ArrowSchema* schema, 
             return rc;
         }
     }
-    x->chunk_rows = (opts && opts->chunk_rows > 0) ? opts->chunk_rows : (int64_t)(4 << 20);
+    x->chunk_rows = (opts && opts->chunk_rows > 0) ? opts->chunk_rows : default_chunk_rows(x->fields);
     x->chunk_rows = (x->chunk_rows + 63) / 64 * 64;
     x->depth = (opts && opts->pipeline_depth > 0) ? opts->pipeline_depth : 3;
     if (x->depth < 2) x->depth = 2;

@@ -4,6 +4,9 @@
 // k_gather_rows moves values of any width outside {1, 2, 4, 8, 16} bytes: the rows of a FixedSizeList column (an
 // embedding of n floats is one 4n-byte value).  It reads every input row once and writes every output byte once; the
 // only extra traffic is the 4-byte d_src entry per row (and the 4-byte iota row K2 scatters to build it).
+//
+// k_gather_bit_rows moves rows of n BITS: the child validity of a FixedSizeList<T, n> with a nullable child, or the values
+// of a FixedSizeList<Boolean, n>.  Output bits [j n, (j + 1) n) are input bits [(in_offset + src[j]) n, ... + n).
 #include <cuda_runtime.h>
 
 #include "dfd_internal.h"
@@ -66,6 +69,34 @@ __global__ void __launch_bounds__(GATHER_BLOCK) k_gather_rows(const uint8_t* __r
     }
 }
 
+// One thread per output 32-bit word: it assembles the word from the (up to 32) row segments it covers, each read with at most
+// two aligned 32-bit loads and one funnel shift, and stores it once.  No atomics, no read-modify-write: every run writes the
+// same words.  A segment is read from the word that holds its first bit and, only when it crosses into it, the word that
+// holds its last bit.  Bits past n_rows x n in the last word are zero.  All bit indices are 64-bit (4 Mi rows x 1024 bits
+// is already 2^32 bits).
+__global__ void __launch_bounds__(GATHER_BLOCK) k_gather_bit_rows(const uint32_t* __restrict__ in, int64_t in_bit0, const uint32_t* __restrict__ src,
+                                                                  int64_t n_rows, int64_t n, uint32_t* __restrict__ out) {
+    const int64_t total = n_rows * n, n_words = (total + 31) >> 5;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < n_words; q += stride) {
+        const int64_t o0 = q << 5, o1 = o0 + 32 < total ? o0 + 32 : total;
+        int64_t j = o0 / n, row_end = (j + 1) * n;
+        uint32_t acc = 0;
+        for (int64_t o = o0; o < o1; ++j, row_end += n) {
+            const int64_t seg_end = row_end < o1 ? row_end : o1;
+            const int len = (int)(seg_end - o);
+            const int64_t s = in_bit0 + (int64_t)__ldg(src + j) * n + (o - (row_end - n));  // first source bit of the segment
+            const int sh = (int)(s & 31);
+            const uint32_t lo = __ldg(in + (s >> 5));
+            const uint32_t hi = sh + len > 32 ? __ldg(in + (s >> 5) + 1) : 0u;
+            const uint32_t v = __funnelshift_r(lo, hi, sh);
+            acc |= (len == 32 ? v : v & ((1u << len) - 1u)) << (int)(o - o0);
+            o = seg_end;
+        }
+        __stcs((unsigned*)out + q, acc);
+    }
+}
+
 namespace {
 
 // enough CTAs to fill every SM once (grid-stride loops do the rest), fewer when the work is small
@@ -101,4 +132,18 @@ int dfd::launch_gather_rows(const void* in, int64_t in_offset, const uint32_t* s
     if ((a & 7) == 0) return launch_rows<uint2>(in, in_offset, src, n_rows, w, out, sm_count, s);
     if ((a & 3) == 0) return launch_rows<uint32_t>(in, in_offset, src, n_rows, w, out, sm_count, s);
     return launch_rows<uint8_t>(in, in_offset, src, n_rows, w, out, sm_count, s);
+}
+
+int dfd::launch_gather_bit_rows(const void* in, int64_t in_offset, const uint32_t* src, int64_t n_rows, int64_t n, void* out, int sm_count,
+                                cudaStream_t s) {
+    if (n_rows <= 0) return DFD_OK;
+    if (n < 1) return set_error(DFD_ERR_INVALID_ARGUMENT, "bit rows of %lld bits", (long long)n);
+    if ((uintptr_t)out & 3) return set_error(DFD_ERR_INVALID_ARGUMENT, "bit-row output must be 4-byte aligned");
+    // the input is read in aligned words: start at the word below it, its leading bytes count as bits
+    const uintptr_t mis = (uintptr_t)in & 3;
+    const int64_t bit0 = in_offset * n + (int64_t)mis * 8;
+    const unsigned grid = gather_grid(k_gather_bit_rows, (n_rows * n + 31) >> 5, sm_count);
+    k_gather_bit_rows<<<grid, GATHER_BLOCK, 0, s>>>((const uint32_t*)((const uint8_t*)in - mis), bit0, src, n_rows, n, (uint32_t*)out);
+    CUDA_TRY(cudaGetLastError(), "k_gather_bit_rows");
+    return DFD_OK;
 }

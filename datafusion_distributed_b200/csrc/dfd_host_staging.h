@@ -153,6 +153,18 @@ inline int64_t split_list_rows_fixed(const int32_t* loff, int32_t w, const uint8
     return ne;
 }
 
+// FixedSizeList<T, n> rows [lo, lo + rows) (lo counts the parent's array offset) over a child at array offset `child_offset`
+// (counted in elements, as every Arrow offset): the child elements they span, child_offset + lo x n onwards, as bits (the
+// child's validity bitmap, or its values when T is Boolean) and as bytes of a child of w bytes per element (w = 0: Boolean).
+struct FslSpan {
+    int64_t first_bit, n_bits;
+    size_t first_byte, n_bytes;
+};
+inline FslSpan fsl_span(int64_t child_offset, int64_t lo, int64_t rows, int64_t n, int64_t w) {
+    const int64_t e0 = child_offset + lo * n, ne = rows * n;
+    return FslSpan{e0, ne, (size_t)(e0 * w), (size_t)(ne * w)};
+}
+
 // Do two flat Arrow arrays hold the same values?  (dictionaries of consecutive batches: readers re-materialise the same
 // dictionary for every batch, and a chunk can keep ONE of them for all its rows.)  `var_ow` = 0 for fixed-width values of
 // `width` bytes (0 = bit-packed booleans), 4 / 8 for Utf8 / Binary / LargeUtf8 offsets.  Buffers follow the Arrow C layout:

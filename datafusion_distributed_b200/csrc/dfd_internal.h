@@ -117,6 +117,7 @@ struct dfd_partitioner {
     enum { LAST_NONE = 0, LAST_DENSE = 1, LAST_REGIONS = 2 } last = LAST_NONE;
     std::vector<dfd_column> last_in, last_out;
     int64_t last_rows = 0, last_stride = 0;
+    bool bit_rows = false;             // accept COL_BIT_ROWS columns (set by the host operator for its own partitioner only)
 };
 
 namespace dfd {
@@ -147,6 +148,7 @@ struct PartitionJob {
     bool gather_wide = false;            // set before prepare(): accept fixed widths outside {1,2,4,8,16} (two-pass local calls)
     struct GatherCol { const void* in; void* out; int64_t in_offset, width; };
     std::vector<GatherCol> gathers;      // wide fixed-width columns, gathered through d_src after K2 (k_gather_rows)
+    std::vector<GatherCol> bit_gathers;  // COL_BIT_ROWS columns (width = bits per row), gathered the same way (k_gather_bit_rows)
     int64_t out_rows = -1;               // rows of the OUTPUT row space (-1: n_rows; single-pass regions: N * region_rows)
     uint32_t* d_hist = nullptr;
     uint32_t* d_base = nullptr;
@@ -194,6 +196,9 @@ int launch_lengths_to_offsets(const void* len, int ow, int64_t n, unsigned long 
 // Gather after K2 through src, the input row of every output row (kernel in dfd_gather.cu): out row j (w bytes) = in row
 // in_offset + src[j], for the fixed widths no scatter instantiation moves.
 int launch_gather_rows(const void* in, int64_t in_offset, const uint32_t* src, int64_t n_rows, int64_t w, void* out, int sm_count, cudaStream_t s);
+// The same for rows of n bits (a bitmap of n_rows x n bits, row r at bit (in_offset + r) x n): out bits [j n, (j + 1) n) = in
+// bits [(in_offset + src[j]) n, ...).  Every output word up to bit n_rows x n is written whole; its bits past the end are zero.
+int launch_gather_bit_rows(const void* in, int64_t in_offset, const uint32_t* src, int64_t n_rows, int64_t n, void* out, int sm_count, cudaStream_t s);
 // Fixed widths the scatter instantiations move; other widths are gathered (two-pass local partition calls only).
 inline bool scatter_width(int64_t w) { return w == 1 || w == 2 || w == 4 || w == 8 || w == 16; }
 
@@ -274,6 +279,10 @@ extern template int launch_scatter_impl<true, ScatterKind::FollowUp>(const Scatt
 // Column kinds that only the host operator hands to hash_columns_locked, never part of the C ABI: Interval(DayTime) (8 bytes)
 // and Interval(MonthDayNano) (16 bytes) dictionary VALUES, hashed field by field like interval keys (KEY_HASH_INTERVAL_*).
 constexpr int32_t COL_INTERVAL_DAY_TIME = 5, COL_INTERVAL_MONTH_DAY_NANO = 6;
+// Payload kind of the host operator's own partitioner (dfd_partitioner::bit_rows), never part of the C ABI: rows of `width`
+// BITS each in a bitmap (`values`, bit 0 of row r at bit (offset + r) x width), moved by k_gather_bit_rows.  The bit rows of a
+// FixedSizeList column: its child's validity, or the values of a Boolean child.  May carry a row validity bitmap.
+constexpr int32_t COL_BIT_ROWS = 7;
 
 // create_hashes over device columns -> raw u64 row hashes (dictionary values, parity hook).  Besides the DFD_COL_* kinds a
 // column may be COL_INTERVAL_DAY_TIME / COL_INTERVAL_MONTH_DAY_NANO.  Caller holds ctx->mu.
