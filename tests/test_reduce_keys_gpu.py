@@ -2,10 +2,11 @@
 compared bit for bit with the exact Python group-by of test_reduce_keys_cpu.py.
 
 Output row order inside a partition is unspecified, so each partition is compared as a set of keys, each with its merged
-states (COUNT, SUM, MIN and MAX over Int64).  Every output buffer starts as FILL bytes with GUARD more past its capacity,
-and every call checks what the reduce must leave alone: offsets past entry G, string bytes past the total, value and
-validity words past row G (and bits at and past G inside the last word, which must be zero), fixed-width bytes past row
-G.  Null keys must come out empty, with their bit clear, whatever lies under them in the input."""
+states (COUNT, SUM, MIN and MAX over Int64).  Every output buffer starts as FILL bytes with GUARD more in front of it and
+past its capacity, and every call checks what the reduce must leave alone: the bytes in front of every buffer, offsets
+past entry G, string bytes past the total, value and validity words past row G (and bits at and past G inside the last
+word, which must be zero), fixed-width bytes past row G.  Null keys must come out empty, with their bit clear, whatever
+lies under them in the input."""
 import ctypes as C
 import uuid
 
@@ -86,31 +87,41 @@ def upload_state(v):
 
 
 def guarded_output(col, n, cap=None, nullable=False):
-    """Output column for `col` with n rows of capacity (var-width: `cap` bytes, default the input's), every byte FILL."""
+    """Output column for `col` with n rows of capacity (var-width: `cap` bytes, default the input's), every byte FILL,
+    each buffer with GUARD more FILL bytes in front of it and behind it (keep holds the whole buffers)."""
     keep, vptr = [], 0
     words = (n + 31) // 32 * 4
+
+    def buf(size):
+        t = cuda_bytes(b"", GUARD + size + GUARD)
+        keep.append(t)
+        return t.data_ptr() + GUARD
+
     if nullable:
-        vt = cuda_bytes(b"", words + GUARD)
-        keep.append(vt)
-        vptr = vt.data_ptr()
+        vptr = buf(words)
     if col.kind in (nv.COL_UTF8, nv.COL_LARGE_UTF8, nv.COL_BINARY):
         ow = 8 if col.kind == nv.COL_LARGE_UTF8 else 4
         cap = col.values_bytes if cap is None else cap
-        ot, dt = cuda_bytes(b"", (n + 1) * ow + GUARD), cuda_bytes(b"", cap + GUARD)
-        keep += [ot, dt]
-        return dfd.DeviceColumn(col.kind, 0, dt.data_ptr(), ot.data_ptr(), vptr, 0, n, keep, col.arrow_type, cap)
-    t = cuda_bytes(b"", (words if col.kind == nv.COL_BOOL else n * col.width) + GUARD)
-    keep.append(t)
-    return dfd.DeviceColumn(col.kind, col.width, t.data_ptr(), 0, vptr, 0, n, keep, col.arrow_type)
+        optr = buf((n + 1) * ow)
+        return dfd.DeviceColumn(col.kind, 0, buf(cap), optr, vptr, 0, n, keep, col.arrow_type, cap)
+    vals = buf(words if col.kind == nv.COL_BOOL else n * col.width)
+    return dfd.DeviceColumn(col.kind, col.width, vals, 0, vptr, 0, n, keep, col.arrow_type)
 
 
 def raw(t):
     return t.cpu().numpy()
 
 
+def past_front_guard(t):
+    """The bytes of a guarded_output buffer from its column's first byte on, after checking the guard in front."""
+    b = raw(t)
+    assert (b[:GUARD] == FILL).all(), "a byte in front of an output buffer was written"
+    return b[GUARD:]
+
+
 def read_bits(t, n, G):
     """Bits of rows [0, G) of a guarded bit-packed output; the rest of the buffer must be as the reduce found it."""
-    b = raw(t)
+    b = past_front_guard(t)
     words = (G + 31) // 32 * 4
     assert (b[words:] == FILL).all(), "a word past row G was written"
     bits = np.unpackbits(b[:words], bitorder="little")
@@ -123,7 +134,7 @@ def read_column(col, n, G):
     valid = read_bits(col.keep[0], n, G) if col.validity else np.ones(G, dtype=bool)
     if col.kind in (nv.COL_UTF8, nv.COL_LARGE_UTF8, nv.COL_BINARY):
         ow = 8 if col.kind == nv.COL_LARGE_UTF8 else 4
-        ob, db = raw(col.keep[-2]), raw(col.keep[-1])
+        ob, db = past_front_guard(col.keep[-2]), past_front_guard(col.keep[-1])
         assert (ob[(G + 1) * ow:] == FILL).all(), "an offset past entry G was written"
         off = ob[:(G + 1) * ow].view(np.int64 if ow == 8 else np.int32).astype(np.int64)
         assert off[0] == 0 and (np.diff(off) >= 0).all()
@@ -140,7 +151,7 @@ def read_column(col, n, G):
         bits = read_bits(col.keep[-1], n, G)
         assert not (bits & ~valid).any(), "a null Boolean key has its value bit set"
         return [bool(b) if v else None for b, v in zip(bits, valid)]
-    b = raw(col.keep[-1])
+    b = past_front_guard(col.keep[-1])
     assert (b[G * col.width:] == FILL).all(), "a value past row G was written"
     vals = b[:G * col.width].view(np.int32 if col.width == 4 else np.int64).tolist()
     return [v if ok else None for v, ok in zip(vals, valid)]

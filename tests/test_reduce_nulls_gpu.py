@@ -103,16 +103,36 @@ def upload(col, valid, off, rng):
     return dfd.DeviceColumn(nv.COL_FIXED, w, t.data_ptr(), 0, vptr, off, len(col), keep)
 
 
-def guarded_output(w, capacity, nullable, bitmap_shift=0):
-    """Output values of `capacity` rows and, when nullable, a bitmap of ceil(capacity / 32) words, both inside FILL bytes
-    with GUARD bytes in front and behind.  -> (DeviceColumn, values tensor, bitmap tensor or None)"""
-    t = torch.full((GUARD + capacity * w + GUARD,), FILL, dtype=torch.uint8, device="cuda")
+def guarded_output(w, capacity, nullable, bitmap_shift=0, value_shift=0):
+    """Output values of `capacity` rows (from `value_shift` bytes past a 64-byte-aligned address) and, when nullable, a
+    bitmap of ceil(capacity / 32) words, both inside FILL bytes with GUARD bytes in front and behind.  -> (DeviceColumn,
+    values tensor, bitmap tensor or None)"""
+    t = torch.full((GUARD + value_shift + capacity * w + GUARD,), FILL, dtype=torch.uint8, device="cuda")
     vt, vptr = None, 0
     if nullable:
         words = (capacity + 31) // 32
         vt = torch.full((GUARD + words * 4 + GUARD,), FILL, dtype=torch.uint8, device="cuda")
         vptr = vt.data_ptr() + GUARD + bitmap_shift
-    return dfd.DeviceColumn(nv.COL_FIXED, w, t.data_ptr() + GUARD, 0, vptr, 0, capacity, [t] + ([vt] if vt is not None else [])), t, vt
+    col = dfd.DeviceColumn(nv.COL_FIXED, w, t.data_ptr() + GUARD + value_shift, 0, vptr, 0, capacity, [t] + ([vt] if vt is not None else []))
+    return col, t, vt
+
+
+def read_output(t, vt, w, G, name, value_shift=0):
+    """Rows [0, G) of a guarded_output: (their bytes as a (G, w) uint8 array, their bits or None), after checking that
+    every byte outside them keeps its fill and that the bits at and past G in the last bitmap word are zero."""
+    raw = t.cpu().numpy()
+    start = GUARD + value_shift
+    assert bool((raw[:start] == FILL).all()) and bool((raw[start + G * w:] == FILL).all()), f"{name}: bytes outside rows [0, {G}) written"
+    vals = raw[start:start + G * w].reshape(G, w)
+    if vt is None:
+        return vals, None
+    rb = vt.cpu().numpy()
+    words = (G + 31) // 32
+    assert bool((rb[:GUARD] == FILL).all()), f"{name}: a byte in front of the output bitmap was written"
+    assert bool((rb[GUARD + words * 4:] == FILL).all()), f"{name}: a bitmap word past row {G} was written"
+    b = np.unpackbits(rb[GUARD:GUARD + words * 4], bitorder="little").astype(bool)
+    assert not b[G:].any(), f"{name}: bits at or past G = {G} are set"
+    return vals, b[:G]
 
 
 def expected_launches(valids, ops, n):
@@ -136,21 +156,10 @@ def run_once(ctx, cols, valids, n_keys, ops, starts_d, N, offsets, out_nullable,
     G = int(out_starts[-1])
     vals, bits = [], []
     for i, (c, (_, t, vt)) in enumerate(zip(cols, outs)):
-        w = width(c)
-        raw = t.cpu().numpy()
-        assert bool((raw[:GUARD] == FILL).all()) and bool((raw[GUARD + G * w:] == FILL).all()), f"column {i}: bytes outside rows [0, {G}) written"
-        v = raw[GUARD:GUARD + G * w].view(np.int64 if c.ndim == 2 else c.dtype)
+        v, b = read_output(t, vt, width(c), G, f"column {i}")
+        v = v.reshape(-1).view(np.int64 if c.ndim == 2 else c.dtype)
         vals.append(v.reshape(G, 2) if c.ndim == 2 else v)
-        if vt is None:
-            bits.append(None)
-            continue
-        rb = vt.cpu().numpy()
-        words = (G + 31) // 32
-        assert bool((rb[:GUARD] == FILL).all()), f"column {i}: a byte in front of the output bitmap was written"
-        assert bool((rb[GUARD + words * 4:] == FILL).all()), f"column {i}: a bitmap word past row {G} was written"
-        b = np.unpackbits(rb[GUARD:GUARD + words * 4], bitorder="little").astype(bool)
-        assert not b[G:].any(), f"column {i}: bits at or past G = {G} are set"
-        bits.append(b[:G])
+        bits.append(b)
     return vals, bits, out_starts
 
 
@@ -222,12 +231,11 @@ def test_every_op_at_null_fraction(ctx, frac):
     reduce_checked(ctx, [gid], [None], states, valids, ALL_OPS, part=gid % 4, N=4, seed=10)
 
 
-def test_min_max_extremes_and_lone_valid_rows(ctx):
-    """Every MIN / MAX op: groups whose one valid row is the first, the last or a random row of the group in input order,
-    groups whose valid rows all hold the op's exact sentinel (the result keeps its bits and its bit), groups where it
-    sits next to other values and nulls, and all-null groups."""
-    rng = np.random.Generator(np.random.PCG64(2))
-    g, size = 3000, 40
+def lone_valid_states(g, size, rng):
+    """g groups of `size` rows in random order, and a column of every MIN / MAX op in which, by (group + column) mod 6,
+    a group's one valid row is its first, its last or a random row in input order, its valid rows (rows 3, 10, 17, ...)
+    all hold the op's exact sentinel, the sentinel sits at row 5 among random valid rows and nulls, or every row is null.
+    Garbage lies under every null.  -> (group id of every row, state columns, their valid arrays)"""
     gid = rng.permutation(np.repeat(np.arange(g), size)).astype(np.int64)
     n = len(gid)
     order = np.argsort(gid, kind="stable")
@@ -245,6 +253,14 @@ def test_min_max_extremes_and_lone_valid_rows(ctx):
         col[put] = sentinel(op)
         states.append(with_nulls(col, valid, op, rng))
         valids.append(valid)
+    return gid, states, valids
+
+
+def test_min_max_extremes_and_lone_valid_rows(ctx):
+    """Every MIN / MAX op: groups whose one valid row is the first, the last or a random row of the group in input order,
+    groups whose valid rows all hold the op's exact sentinel (the result keeps its bits and its bit), groups where it
+    sits next to other values and nulls, and all-null groups."""
+    gid, states, valids = lone_valid_states(3000, 40, np.random.Generator(np.random.PCG64(2)))
     reduce_checked(ctx, [gid], [None], states, valids, MINMAX_OPS, seed=20)
 
 
