@@ -7,17 +7,38 @@ with what the oracle's row order implies, byte for byte: values (junk under null
 string offsets continued across chunks and the dense string bytes."""
 from __future__ import annotations
 
+import os
 import random
+import re
 
 import numpy as np
 
 FILL = 0xAB
 GUARD = 64
+_EXCHANGE_CU = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "datafusion_distributed_b200", "csrc",
+                            "dfd_exchange.cu")
 
 
-def mixed_arrays(n, seed, nulls=True):
+def exchange_constant(name):
+    """A `constexpr int / long long NAME = a * b ...;` of csrc/dfd_exchange.cu."""
+    with open(_EXCHANGE_CU) as f:
+        m = re.search(rf"constexpr\s+(?:int|long long)\s+{name}\s*=\s*([0-9A-Z_ *]+);", f.read())
+    assert m, name
+    v = 1
+    for f in m.group(1).split("*"):
+        f = f.strip()
+        v *= int(f) if f.isdigit() else exchange_constant(f)
+    return v
+
+
+PUSH_THREADS = exchange_constant("PUSH_THREADS")
+BIT_WORDS_PER_CTA = exchange_constant("BIT_WORDS_PER_CTA")  # destination words one k_place_bits CTA covers
+BITS_PER_CTA = 32 * BIT_WORDS_PER_CTA
+
+
+def mixed_arrays(n, seed, nulls=True, binary=False):
     """The mixed schema of tests/test_exchange_gpu.py (Int64, Utf8, LargeUtf8, Boolean, Int32, Float64), typed explicitly so
-    that an all-null or empty column keeps its type."""
+    that an all-null or empty column keeps its type; with `binary`, a nullable Binary column follows."""
     import pyarrow as pa
 
     rnd = random.Random(seed)
@@ -29,7 +50,36 @@ def mixed_arrays(n, seed, nulls=True):
     bl = pa.array([rnd.choice(none + [True, False]) for _ in range(n)], type=pa.bool_())
     i32 = pa.array([rnd.choice(none + [rnd.getrandbits(31)]) for _ in range(n)], type=pa.int32())
     f64 = pa.array(rng.standard_normal(n))
-    return [key, s, ls, bl, i32, f64]
+    if not binary:
+        return [key, s, ls, bl, i32, f64]
+    bn = pa.array([rnd.choice(none + [b"", bytes(rnd.getrandbits(8) for _ in range(rnd.randint(1, 20)))]) for _ in range(n)], type=pa.binary())
+    return [key, s, ls, bl, i32, f64, bn]
+
+
+def fixed_array(typ, n, seed, null_frac=0.0):
+    """n rows of any fixed-width type (Int8 ... Decimal128, MonthDayNano) from random bytes, built at the buffer level."""
+    import pyarrow as pa
+
+    rng = np.random.Generator(np.random.PCG64(seed))
+    data = pa.py_buffer(rng.integers(0, 256, n * (typ.bit_width // 8), dtype=np.uint8).tobytes())
+    validity = pa.py_buffer(np.packbits(rng.random(n) >= null_frac, bitorder="little").tobytes()) if null_frac else None
+    return pa.Array.from_buffers(typ, n, [validity, data])
+
+
+def at_odd_address(a):
+    """The same array, every buffer copied to an odd host address (a numpy byte buffer sliced by 1)."""
+    import pyarrow as pa
+
+    bufs = []
+    for b in a.buffers():
+        if b is None:
+            bufs.append(None)
+            continue
+        raw = np.empty(b.size + 1, dtype=np.uint8)
+        raw[1:] = np.frombuffer(b, dtype=np.uint8)
+        bufs.append(pa.py_buffer(raw[1:]))
+        assert bufs[-1].address % 2 == 1
+    return pa.Array.from_buffers(a.type, len(a), bufs, a.null_count, a.offset)
 
 
 def kind_of(t):
@@ -90,10 +140,10 @@ class HostOut:
     """Output buffers of `cap` rows for `types` (bitmaps as whole 32-bit words); a validity buffer for columns with
     nullable[i]; string columns get nbytes[i] bytes."""
 
-    def __init__(self, types, cap, nullable, nbytes):
+    def __init__(self, types, cap, nullable, nbytes, shift=0):
         import datafusion_distributed_b200 as dfd
 
-        self.types, self.cap, self.bufs, self.cols = types, cap, {}, []
+        self.types, self.cap, self.bufs, self.cols, self.shift = types, cap, {}, [], shift
         for i, t in enumerate(types):
             kind, width = kind_of(t)
             validity = self._buf(i, "validity", _words(cap)) if nullable[i] else 0
@@ -107,7 +157,7 @@ class HostOut:
                 self.cols.append(dfd.DeviceColumn(kind, width, self._buf(i, "values", cap * width), 0, validity, 0, cap, self, t))
 
     def _buf(self, i, what, n):
-        b = np.full(n + GUARD, FILL, dtype=np.uint8)
+        b = np.full(n + GUARD + self.shift, FILL, dtype=np.uint8)[self.shift:]  # (shift = 1: at an odd address)
         self.bufs[(i, what)] = (b, n)
         return b.ctypes.data
 
@@ -134,6 +184,44 @@ def expected_order(dests, n_rows, n_chunks, P, rank=0):
             at += len(idx)
         cps[ch, P] = at
     return (np.concatenate(order) if order else np.zeros(0, np.int64)).astype(np.int64), cps
+
+
+def bit_launches(cps, lanes):
+    """The k_place_bits launches of one dfd_shuffle_host call at world 1, restated from host_push_chunks_locked's compaction:
+    one launch per chunk that delivers rows (when the schema has bitmap lanes: Boolean values and the validity of every
+    nullable column).  Each is (chunk, out_row, runs); a run is (dst_bit, n, fold) in the chunk's output stage, whose word
+    0 is host word out_row >> 5.  Per segment (partition at world 1) with rows and per lane: dst_bit = (out_row & 31) +
+    drow, n = count; when out_row & 31 != 0 and an earlier chunk delivered, a fold run per lane (dst_bit 0, n = out_row & 31)
+    brings in that chunk's bits of the shared host word."""
+    launches, out_row, delivered = [], 0, False
+    for ch in range(cps.shape[0]):
+        counts = np.diff(cps[ch])
+        got = int(counts.sum())
+        if got == 0:
+            continue
+        sh0, drow, runs = out_row & 31, 0, []
+        for c in counts:
+            if c:
+                runs += [(sh0 + drow, int(c), False)] * lanes
+                drow += int(c)
+        if sh0 and delivered:
+            runs += [(0, sh0, True)] * lanes
+        if lanes:
+            launches.append((ch, out_row, runs))
+        delivered, out_row = True, out_row + got
+    return launches
+
+
+def run_words(dst_bit, n):
+    return ((dst_bit & 31) + n + 31) >> 5
+
+
+def run_ctas(dst_bit, n):
+    return -(-run_words(dst_bit, n) // BIT_WORDS_PER_CTA)
+
+
+def launch_ctas(runs):
+    return sum(run_ctas(d, n) for d, n, _ in runs)
 
 
 def verify(out: HostOut, sources, total):

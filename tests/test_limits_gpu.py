@@ -1,6 +1,7 @@
 """GPU parity tests at the 32-bit limits of the C ABI: up to 2^32 - 1 rows per dense call, single-pass regions up to
 N * region_rows = 2^32 - 2 output rows, string offset scans of more than one round (> 2 097 152 rows), LargeUtf8 byte
-offsets past 2^32 and a Utf8 column of exactly 2^31 - 1 bytes; and the argument checks just past each limit.
+offsets past 2^32 and a Utf8 column of exactly 2^31 - 1 bytes, the same two through dfd_shuffle_host, whose string offsets
+continue across chunks; and the argument checks just past each limit.
 
 A row-by-row oracle does not scale to 4 G rows, so the large cases draw keys from a small domain (tests.util
 domain_values) whose destinations the C oracle computes once; on the GPU a row's destination is then LUT[key].
@@ -9,7 +10,10 @@ keeping a cursor per destination, over every column, validity bit and string byt
 swapped unseen, a payload derived from the row id shows a stability error.
 
 Each large case first reads the free device memory and skips, naming the amount, if its budget plus 2 GiB is not free;
-it runs on its own WorkerContext, whose scratch is released with it, and frees its tensors before returning."""
+it runs on its own WorkerContext, whose scratch is released with it, and frees its tensors before returning.  The
+dfd_shuffle_host cases also skip, naming the amount, when the host has too little available memory for their host
+buffers.  On one H100 80GB HBM3 at a 700 W power limit the module takes about 30 s, at most about 44 GiB of device
+memory and 14 GiB of host memory."""
 import gc
 import time
 
@@ -499,3 +503,93 @@ def test_utf8_payload_of_exactly_int32_max_bytes():
     lens[:deficit % n] += 1
     assert int(lens.sum()) == (1 << 31) - 1
     string_case("Utf8 payload of 2^31 - 1 bytes", 5, n, 4, "utf8", lens, 7)
+
+
+# ------------------------------- dfd_shuffle_host: string offsets continued across chunks ----
+
+def host_available():
+    with open("/proc/meminfo") as f:
+        for line in f:
+            if line.startswith("MemAvailable:"):
+                return int(line.split()[1]) * 1024
+    return 0
+
+
+def host_shuffle_string_case(name, gib, host_gib, typ, total, n, n_chunks, seed):
+    """dfd_shuffle_host at world 1 of (int16 key, String of `total` bytes in rows of about 1000 bytes) through
+    Hash([0], 4), in n_chunks chunks through a 448 MiB receive window.  The expected output is the rows of each chunk in
+    (destination, row) order, destination = LUT[key]; offsets, bytes and keys are compared with it on the device."""
+    import uuid
+
+    from tests import host_shuffle_util as H
+
+    if host_available() < host_gib * GiB:
+        pytest.skip(f"{name} needs {host_gib} GiB of available host memory, {host_available() / GiB:.1f} GiB is available")
+    P = 4
+    odt, kind = (np.int64, pa.large_string()) if typ == "large" else (np.int32, pa.string())
+    with Budget(name, gib) as bud:
+        ctx = dfd.WorkerContext(0)
+        g = torch.Generator(device="cuda").manual_seed(seed)
+        key = torch.randint(-(1 << 15), 1 << 15, (n,), dtype=torch.int16, device="cuda", generator=g)
+        lens = torch.randint(950, 1050, (n,), dtype=torch.int64, device="cuda", generator=g)
+        deficit = total - int(lens.sum())
+        lens += deficit // n
+        lens[:deficit % n] += 1
+        assert int(lens.sum()) == total and int(lens.min()) > 0
+        off = torch.zeros(n + 1, dtype=torch.int64, device="cuda")
+        torch.cumsum(lens, 0, out=off[1:])
+        data = np.empty(total, dtype=np.uint8)
+        host_data = torch.from_numpy(data)
+        step = 1 << 15
+        for a in range(0, n, step):
+            b = min(n, a + step)
+            host_data[int(off[a]):int(off[b])].copy_(string_bytes(rows(a, b), lens[a:b]))
+        key_h = key.cpu().numpy()
+        arrays = [pa.array(key_h), pa.Array.from_buffers(kind, n, [None, pa.py_buffer(off.cpu().numpy().astype(odt)), pa.py_buffer(data)])]
+        out = H.HostOut([a.type for a in arrays], n, [False, False], {1: total})
+        ex = dfd.ShuffleExchange(ctx, 0, 1, None)
+        ex.setup_window(448 << 20)
+        node = dfd.NetworkShuffleExec.try_new(dfd.Partitioning.Hash([0], P), uuid.uuid4(), 1, 1, 1)
+        cps = node.shuffle_host(ex, H.in_columns(arrays, n), n, n_chunks, out.cols, n)
+        bud.sample()
+        ex.close()
+        ctx.close()
+        del arrays, host_data, data
+        # expected: chunk by chunk, rows by destination in input order
+        lut = lut_of("i16", P)
+        dest = lut[key_index(key)].long()
+        chunk = torch.zeros(n, dtype=torch.int64, device="cuda")
+        for i in range(1, n_chunks):
+            chunk[n * i // n_chunks:] += 1
+        order = torch.sort(chunk * P + dest, stable=True).indices
+        w = torch.searchsorted((chunk * P + dest)[order], torch.arange(n_chunks * P + 1, device="cuda")).cpu().numpy()
+        assert np.array_equal(cps, np.stack([w[ch * P:ch * P + P + 1] for ch in range(n_chunks)]))
+        kb, _ = out.bufs[(0, "values")]
+        assert torch.equal(torch.from_numpy(kb[:2 * n].view(np.int16)).cuda(), key[order])
+        want_off = torch.zeros(n + 1, dtype=torch.int64, device="cuda")
+        torch.cumsum(lens[order], 0, out=want_off[1:])
+        ob, _ = out.bufs[(1, "offsets")]
+        got_off = torch.from_numpy(ob[:(n + 1) * np.dtype(odt).itemsize].view(odt)).cuda().to(torch.int64)
+        assert torch.equal(got_off, want_off), "output offsets"
+        assert int(got_off[-1]) == total
+        vb, _ = out.bufs[(1, "values")]
+        for a in range(0, n, step):
+            b = min(n, a + step)
+            lo, hi = int(want_off[a]), int(want_off[b])
+            assert torch.equal(torch.from_numpy(vb[lo:hi]).cuda(), string_bytes(order[a:b], lens[order[a:b]])), f"bytes of output rows [{a}, {b})"
+        for b, cap in out.bufs.values():
+            assert (b[cap:] == H.FILL).all()
+        del key, lens, off, dest, chunk, order, want_off, got_off, out
+    return cps
+
+
+def test_host_shuffle_utf8_of_exactly_int32_max_bytes():
+    """A Utf8 output of exactly 2^31 - 1 bytes delivered in 8 chunks: the int32 offsets continue across chunks up to a
+    last offset of INT32_MAX, which the per-chunk check (need > INT32_MAX) accepts.  (At world 1 a Utf8 input cannot
+    hold more, so the refusal one byte past needs two producers.)"""
+    host_shuffle_string_case("dfd_shuffle_host, Utf8 of 2^31 - 1 bytes", 3, 6, "utf8", (1 << 31) - 1, 1 << 21, 8, 8)
+
+
+def test_host_shuffle_large_utf8_past_4_gib():
+    """A LargeUtf8 output of 2^32 + 2^28 bytes in 16 chunks: the int64 offsets, re-based chunk by chunk, pass 2^32."""
+    host_shuffle_string_case("dfd_shuffle_host, LargeUtf8 past 4 GiB", 3, 12, "large", (1 << 32) + (1 << 28), (1 << 22) + 4_099, 16, 9)

@@ -143,10 +143,10 @@ def test_peer_aligned_constructed_runs(ctx, P, fast):
     arrays = schema(keys_for_counts(cnt, pool, seed=P))
     assert np.array_equal(exchange_starts(ctx, arrays, [0], P, window), starts)  # (the same stride for these rows)
     ring = 8  # (the Decimal128 column makes the widest column 16 bytes: an 8-byte ring)
-    fallbacks, ran = profiled(lambda: check_exchange(ctx, arrays, [0], P, window=window))
+    fallbacks, ran = profiled(ctx, lambda: check_exchange(ctx, arrays, [0], P, window=window))
     assert fallbacks == 0
     assert_ran(ran, targets(1, fast, [ring], True, P))
-    _, ran = profiled(lambda: check_exchange(ctx, arrays, [0], P, fused=True, window=window))
+    _, ran = profiled(ctx, lambda: check_exchange(ctx, arrays, [0], P, fused=True, window=window))
     assert_ran(ran, targets(0, fast, [8, 4, 16] if fast else [2, 4, 16], True, P))
 
 
@@ -264,7 +264,7 @@ def test_local_constructed_runs(ctx, name, layout, schema):
     idx = keys_for_counts(cnt, pool_of(schema, N), seed=N * 7 + delta)
     arrays, key_cols = table(schema, N, idx, seed=N + delta)
     if layout in ("exact_odd", "minus1_sync"):
-        _, ran = profiled(lambda: run_local(ctx, arrays, key_cols, N, rr, rerun, sync))
+        _, ran = profiled(ctx, lambda: run_local(ctx, arrays, key_cols, N, rr, rerun, sync))
         assert_ran(ran, instantiations(schema, arrays, N))
     else:
         run_local(ctx, arrays, key_cols, N, rr, rerun, sync)
